@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py — the hot path's headline benchmark (BASELINE.json: "GFLOP/s at N=K=M=16384 fp32").
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--workload NAME]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--workload NAME] [--dump-outputs DIR]
 
 One step = one MatrixMultiplicationKernel invocation C = A * B (operand preparation + GEMM, or the
 configured semiring) over one batch of synthetic matrices through the C-ABI of libmm_b200.so.
@@ -17,6 +17,10 @@ Printed JSON line (rank 0): see the contract in the task statement; in addition
   e2e           the same metric through ONE host-pointer call for the whole problem, H2D + D2H inside: mm_gemm_host()
                 at N = 1, mm_multi_gemm_host() over all N GPUs (issued by rank 0) at N > 1
 `--impl reference` times only the reference CPU path (oracle/_ref; the oracle port if absent).
+`--dump-outputs DIR` writes what the last timed step computed: DIR/c.npy (DIR/c_rank<r>.npy per rank when N > 1),
+C in float32 (float64 for double), on a fixed, seeded sample of whole rows when C is larger than 48 MiB, and
+DIR/c_rows.npy, the indices of those rows (float64).  The inputs are seeded: two builds given the same arguments
+compute from identical matrices and can be compared output for output.
 """
 import argparse
 import ctypes
@@ -33,11 +37,11 @@ sys.path.insert(0, ROOT)
 
 WORKLOADS = {
     # name: (dtype name, map, reduce, n, k, m, BASELINE.json config it is)
-    "float16384": ("float", "Multiply", "Add", 16384, 16384, 16384, "configs[1] float 16384^3 tcgen05"),
+    "float16384": ("float", "Multiply", "Add", 16384, 16384, 16384, "configs[1] float 16384^3 wgmma tf32"),
     "half32768": ("half", "Multiply", "Add", 32768, 32768, 32768, "configs[2] half 32768^3"),
     "double8192": ("double", "Multiply", "Add", 8192, 8192, 8192, "configs[3] double 8192^3"),
     "addmin8192": ("float", "Add", "Min", 8192, 8192, 8192, "configs[4] (add,min) float 8192^3"),
-    "uint8_16384": ("uint8_t", "Multiply", "Add", 16384, 16384, 16384, "SURVEY.md 8(f3): uint8_t on tcgen05 kind::i8"),
+    "uint8_16384": ("uint8_t", "Multiply", "Add", 16384, 16384, 16384, "SURVEY.md 8(f3): uint8_t on the integer tensor cores"),
     "half8192": ("half", "Multiply", "Add", 8192, 8192, 8192, "experiments: with --flags 2 the bit-exact half datapath the half host programs run"),
     "float4096": ("float", "Multiply", "Add", 4096, 4096, 4096, "reduced size, debugging only"),
 }
@@ -50,7 +54,8 @@ def load_peaks():
         p = json.load(open(path))
         p["_source"] = "measured"
         return p
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "_source": "fallback"}
+    # NVIDIA H100 SXM data sheet (700 W card), dense: 3.35 TB/s HBM3, 989 TFLOP/s BF16
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "_source": "H100 SXM data sheet"}
 
 
 class ClockSampler:
@@ -207,8 +212,7 @@ def host_threads():
 
     Naive<> walks a column of B with a stride of M elements: 16384 cache lines (1 MiB) per output element,
     reused by the next 15 columns.  That working set fits one core's private L2 once, not twice, so two
-    hyper-threads on a core evict each other (on the 128-thread host of the B200 boxes a float 16384^2 step
-    with one row on each of the 128 logical CPUs did not finish within 45 s; one row on one thread takes 5 s)."""
+    hyper-threads on a core evict each other."""
     try:
         allowed = set(os.sched_getaffinity(0))
     except (AttributeError, OSError):
@@ -290,7 +294,7 @@ def cpu_sample_text(rows, k, cols, threads):
 
 
 def cpu_baseline_line(dtype_name, mp_name, rd_name, unit, k, m, a_rows_of, b):
-    """The `cpu_baseline` object of the B200 arm: the reference's Naive<> on the same bounded sample the
+    """The `cpu_baseline` object of the GPU arm: the reference's Naive<> on the same bounded sample the
     reference arm times — one row of C per physical core, first SAMPLE_COLS columns, full K."""
     threads = host_threads()
     a_rows, b_s, cols = cpu_sample_inputs(None, k, m, threads, a_rows=a_rows_of(threads), b=b)
@@ -312,6 +316,8 @@ def main():
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--flags", type=int, default=0, help="MM_FLAG_* bits (debugging)")
     ap.add_argument("--tune", default="", help="comma-separated knob=value pairs for mm_context_set_tuning (sweeps)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the last timed step's C (or a seeded row sample of it) as .npy files into DIR")
     ap.add_argument("--emulate-ranks", type=int, default=0,
                     help="experiments only: time ONE rank's row-block of an R-GPU split on this GPU (N/R rows); "
                          "the printed value is that block's own rate, not a multi-GPU figure")
@@ -336,7 +342,7 @@ def main():
               "partition": ("C blocks over a %d x %d grid of %d GPU(s): %d row-block(s) x %d column-block(s); a rank holds (and "
                             "prepares, every step) its A row-block and its B column-block; no collective inside a step"
                             % (grid_r, grid_c, args.gpus, grid_r, grid_c)),
-              "l2": "inputs (A+B+C = %.2f GB) far larger than the 126 MB L2; no explicit flush" %
+              "l2": "inputs (A+B+C = %.2f GB) far larger than the 50 MB L2; no explicit flush" %
                     (1e-9 * {"float": 4, "half": 2, "double": 8, "uint8_t": 1}[dtype_name] * (N * K + K * M + N * M))}
 
     import numpy as np
@@ -371,13 +377,13 @@ def main():
             "gpu_launches": 0}))
         return 0
 
-    # ------------------------------------------------------------------ B200 arm
+    # ------------------------------------------------------------------ GPU arm
     import torch
     import torch.distributed as dist
     import gemm_hls_b200 as G
 
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py: no CUDA device — the B200 path has no CPU fallback")
+        raise SystemExit("bench.py: no CUDA device — the GPU path has no CPU fallback")
     torch.cuda.set_device(local_rank)
     dev = torch.device("cuda", local_rank)
     host_group = None
@@ -480,6 +486,8 @@ def main():
     prep_s, main_s, calls = ctx.profile_read()
     ctx.set_profiling(False)
     clocks = sampler.stop(t_begin, t_end) if sampler else None
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, c_blk, "c" if world == 1 else "c_rank%d" % rank)
 
     t_max = torch.tensor([elapsed_ms], device=dev, dtype=torch.float64)
     if world > 1:
@@ -513,46 +521,32 @@ def main():
         path = G.kernel_path(dtype, mp, rd, flags)
         main_avg_s = main_s / max(calls, 1)
         local_ops = 2.0 * n_local * K * m_local
-        if path in ("tcgen05_tf32", "tcgen05_f16", "tcgen05_i8"):
+        if path in ("wgmma_tf32", "wgmma_f16", "wgmma_i8"):
             # burst figure when the whole timed region is shorter than the ~1 s it takes the power
             # cap to pull the clocks down, the sustained one for a seconds-long back-to-back loop
             long_run = elapsed_ms > 1500.0
             peak_bf16 = peaks.get("bf16_tflops_sustained", peaks["bf16_tflops"]) if long_run else peaks["bf16_tflops"]
-            peak = {"tcgen05_tf32": peak_bf16 / 2.0, "tcgen05_f16": peak_bf16, "tcgen05_i8": peak_bf16 * 2.0}[path]
+            peak = {"wgmma_tf32": peak_bf16 / 2.0, "wgmma_f16": peak_bf16, "wgmma_i8": peak_bf16 * 2.0}[path]
             peak_note = ("%s bf16 %s %.1f TF/s%s" % (peaks["_source"], "sustained" if long_run else "burst", peak_bf16,
-                         {"tcgen05_tf32": " / 2 (kind::tf32 issues at half the 16-bit rate)", "tcgen05_f16": "",
-                          "tcgen05_i8": " x 2 (kind::i8 issues at twice the 16-bit rate; no measured int8 figure in "
-                                        "MEASURED_PEAKS.json)"}[path]))
+                         {"wgmma_tf32": " / 2 (tf32 wgmma issues at half the 16-bit rate)", "wgmma_f16": "",
+                          "wgmma_i8": " x 2 (8-bit wgmma issues at twice the 16-bit rate)"}[path]))
             roof = {"bound": "tensor", "achieved": 1e-12 * local_ops / main_avg_s, "peak": peak, "unit": "TFLOP/s"}
         elif path == "dmma_f64":
-            # FP64 DMMA is not in MEASURED_PEAKS.json.  Measured on this pool with a registers-only DMMA loop
-            # (scripts/exp_fp64_pipes.cu, profiles/r01_exp_fp64_pipes.jsonl): 37.05-37.13 TF/s at 1965 MHz
-            # = 64 FMA/clk/SM; the HGX B200 datasheet's 296 TF / 8 GPUs = 37 TF/s.
-            peak = 37.1
-            peak_note = ("FP64 tensor (DMMA) 37.1 TF/s: registers-only DMMA loop measured on this pool "
-                         "(profiles/r01_exp_fp64_pipes.jsonl); datasheet 37; not in MEASURED_PEAKS.json")
+            # FP64 DMMA is not in MEASURED_PEAKS.json: the H100 SXM data sheet's FP64 tensor-core figure
+            peak = 67.0
+            peak_note = "FP64 tensor (DMMA) 67 TF/s: H100 SXM data sheet (700 W card); not measured"
             roof = {"bound": "tensor", "achieved": 1e-12 * local_ops / main_avg_s, "peak": peak, "unit": "TFLOP/s"}
         else:
             peak, peak_note = semiring_peak(dtype_name, mp_name, rd_name, flags)
             roof = {"bound": "cuda_core_issue", "achieved": 1e-12 * local_ops / main_avg_s, "peak": peak, "unit": "TOp/s"}
-            if peak == 74.4:
-                roof["frac_of_measured_mix"] = roof["achieved"] / 52.5
         roof["frac"] = roof["achieved"] / roof["peak"]
         roof["kernel"] = path
         roof["kernel_ms"] = 1e3 * main_avg_s
         roof["prep_ms"] = 1e3 * prep_s / max(calls, 1)
-        roof["prep_note"] = ("exposed operand preparation before the main kernel starts (A's TF32 rounding); B's rounding "
-                             "runs concurrently with the GEMM and is inside kernel_ms" if path == "tcgen05_tf32" else "")
+        roof["prep_note"] = ("operand preparation before the main kernel starts: B transposed into its K-major copy "
+                             "(rounded to TF32 for float), A rounded to TF32 for float" if path.startswith("wgmma") else "")
         roof["peak_source"] = peak_note
-        # DRAM bytes of the dominant kernel: only a figure MEASURED for exactly this workload, GPU count and
-        # default tuning (one `ncu --set full` capture per round, profiles/ncu_traffic.json); null otherwise
         roof["algorithmic_bytes"] = es * (n_local * K + K * m_local + n_local * m_local)
-        traffic = None
-        tr_path = os.path.join(ROOT, "profiles", "ncu_traffic.json")
-        if os.path.exists(tr_path) and not tune and flags == 0:
-            traffic = json.load(open(tr_path)).get("%s@%s@n%d" % (path, args.workload, world))
-        roof["traffic"] = traffic
-        roof["traffic_ratio"] = (traffic / roof["algorithmic_bytes"]) if traffic else None
 
         out = {"metric": metric_name, "value": value, "unit": metric, "n_gpus": world, "steps": args.steps,
                "warmup": args.warmup, "ms_per_step": ms_per_step, "higher_is_better": True, "scaling": "strong",
@@ -641,21 +635,32 @@ def main():
 
 def semiring_peak(dtype_name, mp_name, rd_name, flags):
     """Derived CUDA-core issue ceiling (DESIGN.md 3.3): one warp instruction per clock and scheduler
-    = 148 SMs x 4 x 32 lanes x 1.965 GHz = 37.2e12 lane-instructions/s, 2 ops per element-step.
-      float (Add, Min|Max): 1 FADD2 + 1 FMNMX3 per two element-steps = 1.0 slot per step -> 74.4 TOp/s.  MEASURED
-        (scripts/exp_pipe_rates.cu, profiles/r02_exp_semiring.md): each of the two instructions alone issues every
-        cycle, but their mix needs 1.38 cycles per instruction (1.42 with the kernel's fragment loads): the ceiling this
-        instruction mix can reach is 52.5 TOp/s.  `peak` stays the derived 74.4 so that rounds compare; `frac_of_measured_mix`
-        is printed beside it.
-      anything else (e.g. float (Multiply, Add) under MM_FLAG_EXACT: 1 FMUL2 per two steps + 1 FADD per step):
-        1.5 slots per step -> 49.6"""
-    fast_minmax = dtype_name == "float" and mp_name == "Add" and rd_name in ("Min", "Max") and not (flags & 2)
-    peak = 74.4 if fast_minmax else 49.6
-    note = ("derived CUDA-core issue ceiling at 1965 MHz, %s (DESIGN.md 3.3); neither HBM- nor tensor-bound%s"
-            % ("1 FADD2 + 1 FMNMX3 per two element-steps" if fast_minmax else "1.5 issue slots per element-step",
-               "; measured ceiling of that instruction mix incl. fragment loads: 52.5 TOp/s (profiles/r02_exp_semiring.md)"
-               if fast_minmax else ""))
+    = 132 SMs x 4 x 32 lanes x 1.98 GHz (H100 SXM maximum boost clock) = 33.5e12 lane-instructions/s.  Every
+    element-step is one Map and one Reduce instruction (2 ops in 2 issue slots): 33.5 TOp/s."""
+    peak = 33.5
+    note = "derived CUDA-core issue ceiling at 1980 MHz, 2 issue slots per element-step (DESIGN.md 3.3); not measured"
     return peak, note
+
+
+DUMP_BYTES = 48 << 20   # sample budget of --dump-outputs (whole rows of C)
+
+
+def dump_outputs(out_dir, c, name):
+    """C (a device tensor) as float32 / float64 .npy; a fixed, seeded sample of whole rows when it is larger than
+    DUMP_BYTES, with the sampled row indices beside it."""
+    import numpy as np
+    import torch
+    out_t = torch.float64 if c.dtype == torch.float64 else torch.float32
+    rows, cols = c.shape
+    per_row = cols * (8 if out_t == torch.float64 else 4)
+    if rows * per_row <= DUMP_BYTES:
+        idx = np.arange(rows)
+    else:
+        idx = np.sort(np.random.default_rng(1234).choice(rows, size=max(1, DUMP_BYTES // per_row), replace=False))
+    os.makedirs(out_dir, exist_ok=True)
+    sel = c[torch.from_numpy(idx).to(c.device)].to(out_t).cpu().numpy()
+    np.save(os.path.join(out_dir, name + ".npy"), sel)
+    np.save(os.path.join(out_dir, name + "_rows.npy"), idx.astype(np.float64))
 
 
 if __name__ == "__main__":

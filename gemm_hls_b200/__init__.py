@@ -1,8 +1,8 @@
-"""gemm_hls_b200 — B200-native MatrixMultiplication hot path of spcl/gemm_hls.
+"""gemm_hls_b200 — H100-native (sm_90a) MatrixMultiplication hot path of spcl/gemm_hls.
 
 Thin ctypes binding over the C-ABI library ``libmm_b200.so`` (include/mm_b200.h).  The product is
 the CUDA library; this module only loads it and passes pointers.  There is no CPU fallback: if the
-library is missing or no B200 is present the calls raise.
+library is missing or no H100 is present the calls raise.
 
 Reference surface mirrored here (file:line under the reference checkout):
   * ``MatrixMultiplicationKernel(a, b, c, n, k, m)``  include/MatrixMultiplication.h:155-171
@@ -16,7 +16,7 @@ import os
 import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-# MM_B200_LIB: A/B experiments load a variant build (scripts/build_semiring_variants.sh); the product is the in-tree library
+# MM_B200_LIB: A/B experiments load a variant build of the library; the product is the in-tree library
 LIB_PATH = os.environ.get("MM_B200_LIB") or os.path.join(HERE, "libmm_b200.so")
 
 # MM_DATA_TYPE codes

@@ -1,6 +1,6 @@
 // C-ABI of libmm_b200.so (include/mm_b200.h): context / buffer lifecycle mirroring the
 // hlslib::ocl calls of host/RunHardware.cpp:116-190, the dispatch of one
-// MatrixMultiplicationKernel invocation onto the B200 kernel families, the pipelined host-pointer
+// MatrixMultiplicationKernel invocation onto the sm_90a kernel families, the pipelined host-pointer
 // entry (test/TestSimulation.cpp:66) and its row-block split over the GPUs of one box.
 #include <algorithm>
 #include <chrono>
@@ -114,7 +114,7 @@ bool valid_op(int o) { return o >= 0 && o < MM_OP_COUNT; }
 
 enum Path { kPathTcgen05, kPathDmma, kPathSemiring };
 
-// uint8_t on tcgen05 kind::i8: products accumulate exactly in 32-bit integers while 255^2 * K < 2^31; the low byte
+// uint8_t on the integer tensor cores: products accumulate exactly in 32-bit integers while 255^2 * K < 2^31; the low byte
 // of the exact sum is the reference's modulo-256 arithmetic.  Longer K takes the CUDA-core kernel.
 constexpr unsigned kMaxKInt8Tensor = 33024;
 
@@ -660,8 +660,8 @@ int mm_context_create(int device, mm_context **out) {
   MM_CUDA_TRY(cudaSetDevice(device));
   cudaDeviceProp prop;
   MM_CUDA_TRY(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10) {
-    return fail(MM_ERR_UNSUPPORTED, std::string("libmm_b200 is built for sm_100a only; device is sm_") +
+  if (prop.major != 9 || prop.minor != 0) {
+    return fail(MM_ERR_UNSUPPORTED, std::string("libmm_b200 is built for sm_90a only; device is sm_") +
                                         std::to_string(prop.major) + std::to_string(prop.minor));
   }
   mm_context *ctx = new mm_context();
@@ -837,7 +837,7 @@ int mm_kernel_launch_count(int dtype, int map_op, int reduce_op, int flags) {
 const char *mm_kernel_path(int dtype, int map_op, int reduce_op, int flags) {
   if (!valid_dtype(dtype) || !valid_op(map_op) || !valid_op(reduce_op)) return "invalid";
   switch (select_path(dtype, map_op, reduce_op, flags, 2, 64)) {
-    case kPathTcgen05: return dtype == MM_DTYPE_FLOAT ? "tcgen05_tf32" : (dtype == MM_DTYPE_UINT8 ? "tcgen05_i8" : "tcgen05_f16");
+    case kPathTcgen05: return dtype == MM_DTYPE_FLOAT ? "wgmma_tf32" : (dtype == MM_DTYPE_UINT8 ? "wgmma_i8" : "wgmma_f16");
     case kPathDmma: return "dmma_f64";
     case kPathSemiring: return "semiring_simt";
   }

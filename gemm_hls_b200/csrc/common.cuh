@@ -31,9 +31,9 @@ struct Scratch {
   size_t bytes = 0;
 };
 
-// Run-time tuning of the kernel families: the B200 counterpart of the reference's CMake-time tile /
-// parallelism knobs (CMakeLists.txt:17-29), swept by scripts/tile_sweep.py the way
-// scripts/build_manager.py:224-306 sweeps builds.  One instance per context: defaults, then the
+// Run-time tuning of the kernel families: the GPU counterpart of the reference's CMake-time tile /
+// parallelism knobs (CMakeLists.txt:17-29), selected at run time where
+// scripts/build_manager.py:224-306 rebuilds.  One instance per context: defaults, then the
 // MM_TUNE_* environment variables read ONCE at mm_context_create(), then mm_context_set_tuning().
 // Indexed by the MM_TUNE_* codes of include/mm_b200.h.
 struct Tuning {
@@ -80,10 +80,9 @@ struct GemmArgs {
 // CUDA-core semiring tile kernel, any (dtype, map, reduce).  semiring_*.cu
 int launch_semiring(int dtype, int map_op, int reduce_op, const GemmArgs &args);
 
-// tcgen05 tensor-core GEMM for (Multiply, Add) float (kind::tf32) and half (kind::f16).
+// wgmma tensor-core GEMM for (Multiply, Add) float (tf32), half (f16) and uint8_t (u8).
 // The context's scratch holds, in this order: [B operand copy][A operand copy][counters].
-//   B operand copy: float = B rounded to TF32 (same row-major K x M layout when the kernel reads B
-//     MN-major, the transposed M x K copy otherwise); half = nothing when B is read in place.
+//   B operand copy: the transposed M x K copy wgmma reads K-major, rounded to TF32 for float.
 //   A operand copy: float = A rounded to TF32; any type with MM_FLAG_TRANSPOSED_A = A transposed.
 size_t tcgen05_scratch_bytes(int dtype, unsigned n, unsigned k, unsigned m, int flags, const Tuning &t);
 size_t tcgen05_bt_bytes(int dtype, unsigned k, unsigned m, int flags, const Tuning &t);  // = offset of the A copy

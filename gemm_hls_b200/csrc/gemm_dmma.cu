@@ -1,8 +1,8 @@
 // Tensor-core path for the dense (Multiply, Add) contraction on double:  C = A * B  in FP64.
-// tcgen05 has no f64 kind, so this is the warp-level DMMA instruction
-// mma.sync.aligned.m8n8k4.row.col.f64 (the only FP64 shape sm_100a executes natively; the larger
+// wgmma has no f64 kind, so this is the warp-level DMMA instruction
+// mma.sync.aligned.m8n8k4.row.col.f64 (the only FP64 shape sm_90a executes natively; the larger
 // PTX shapes are split into it) fed from a TMA shared-memory ring.
-// B200 counterpart of the reference's PE chain for MM_DATA_TYPE=double
+// sm_90a counterpart of the reference's PE chain for MM_DATA_TYPE=double
 // (kernel/Compute.cpp:53-146; README.md:8 quotes 132 GFLOP/s for it on a VCU1525).
 //
 // CTA tile BM x 128 (BM = 128, or 64 for short row blocks), BK = 32, 3 stages.  Eight compute warps as
@@ -11,11 +11,8 @@
 // handed over through mbarriers (full[s]: TMA transaction bytes; empty[s]: one arrival per compute
 // warp), so compute warps never meet at a block-wide barrier.
 //
-// How it got here (profiles/r01_exp_fp64_pipes.jsonl, r01_exp_dmma_lds.jsonl, r01_exp_dmma_ws*.log):
-// the LDS + DMMA loop alone runs at the pipe peak (37.1 TF/s); with every warp issuing its share of a
-// cp.async (LDGSTS) prefetch the kernel stayed at 32.4 TF/s, with one / four dedicated LDGSTS producer
-// warps at 31.8 / 35.1, with the loads switched off at 36.5.  TMA removes the LSU instructions and the
-// address arithmetic altogether: 36.2 TF/s on 8192^3 (cuBLAS: 35.5).
+// The loads are TMA rather than cp.async (LDGSTS) issued by the compute warps: TMA removes the LSU
+// instructions and the address arithmetic from the warps that feed the DMMA pipe.
 #include <cuda_runtime.h>
 
 #include <cmath>
@@ -23,7 +20,7 @@
 #include <cstdint>
 
 #include "common.cuh"
-#include "ptx_sm100.cuh"
+#include "ptx_sm90.cuh"
 #include "tma_host.cuh"
 
 namespace mm {
@@ -213,11 +210,11 @@ int launch_dmma(const GemmArgs &g) {
   }
   if (!get_encode_fn()) return fail(MM_ERR_CUDA, "cuTensorMapEncodeTiled entry point not available");
   // Tile height: 128 rows per CTA, or 64 when the 128-row tiling leaves the last wave mostly empty
-  // (e.g. a 1024-row block of the 8-GPU split of 8192^3: 512 tiles on 148 SMs = 3.46 waves; 1024
-  // half-height tiles = 6.92 waves of half the duration).  The half-height tile reads B twice as
+  // (e.g. a 640-row block of 8192 columns: 320 tiles on 132 SMs = 2.42 waves; 640 half-height tiles
+  // = 4.85 waves of half the duration).  The half-height tile reads B twice as
   // often per output row and runs ~2 % below the full tile, so it has to win by more than 5 %.
   // The tuning knob MM_TUNE_DMMA_TILE_ROWS (64 | 128) forces one of them.
-  int sms = 148, dev = 0;
+  int sms = 132, dev = 0;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const double t128 = double(ceil_div(g.n, 128)) * ceil_div(g.m, BN), t64 = double(ceil_div(g.n, 64)) * ceil_div(g.m, BN);

@@ -131,7 +131,7 @@ struct Max {  // Operators.h:89-100 — identity is numeric_limits<T>::min() as 
   static __device__ __forceinline__ T identity() { return Lim<T>::min_value(); }
 };
 
-// Hardware min / max for float (FMNMX, and FMNMX3 when the compiler fuses two reductions): one
+// Hardware min / max for float (FMNMX): one
 // instruction instead of the compare + select that the literal `(a < b) ? a : b` needs.  Identical
 // results for all finite inputs except the sign of a zero when the operands are -0 and +0, and
 // NaNs are dropped instead of propagated; selected for float unless MM_FLAG_EXACT is given.
@@ -148,46 +148,6 @@ template <>
 struct MaxFast<float> {
   static __device__ __forceinline__ float Apply(float a, float b) { return fmaxf(a, b); }
   static __device__ __forceinline__ float identity() { return Lim<float>::min_value(); }
-};
-
-// ---- packed pairs (float) ------------------------------------------------------------------------
-// Blackwell issues two IEEE round-to-nearest FP32 additions / multiplications in ONE instruction
-// (add.rn.f32x2 / mul.rn.f32x2 -> FADD2 / FMUL2; a scalar operand is broadcast for free), each half
-// rounded exactly like __fadd_rn / __fmul_rn.  The tile kernel uses them for two adjacent columns
-// of C at a time, which halves the issue slots of a float Map (and of a float Sum / Product Reduce)
-// without touching the per-element order of operations.
-struct F32x2 {
-  unsigned long long v;
-};
-__device__ __forceinline__ F32x2 pack_f32x2(float lo, float hi) {
-  F32x2 r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r.v) : "f"(lo), "f"(hi));
-  return r;
-}
-__device__ __forceinline__ void unpack_f32x2(F32x2 p, float &lo, float &hi) {
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(p.v));
-}
-template <class Op>
-struct PackedOp {
-  static constexpr bool value = false;
-};
-template <>
-struct PackedOp<Sum<float>> {
-  static constexpr bool value = true;
-  static __device__ __forceinline__ F32x2 Apply2(F32x2 a, F32x2 b) {
-    F32x2 r;
-    asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r.v) : "l"(a.v), "l"(b.v));
-    return r;
-  }
-};
-template <>
-struct PackedOp<Product<float>> {
-  static constexpr bool value = true;
-  static __device__ __forceinline__ F32x2 Apply2(F32x2 a, F32x2 b) {
-    F32x2 r;
-    asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r.v) : "l"(a.v), "l"(b.v));
-    return r;
-  }
 };
 
 // ---- packed pairs (half) -------------------------------------------------------------------------

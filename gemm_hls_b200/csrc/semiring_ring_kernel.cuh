@@ -2,8 +2,7 @@
 // BOTH tiles arrive by TMA into a 4-stage ring, stages are handed over through mbarriers (full: TMA
 // transaction bytes; empty: one arrival per warp), and there is no block-wide barrier in the main loop.
 //
-// Why: the inner loop of semiring_tile_kernel alone runs at 44.8 TOp/s for float (Add, Min), the kernel at
-// 39.9 (profiles/r01_exp_semiring_issue.jsonl): the difference is the per-k-tile __syncthreads (every 16
+// Why: what separates semiring_tile_kernel from its inner loop alone is the per-k-tile __syncthreads (every 16
 // k-steps), the LDG + transposing STS of the A tile and its address arithmetic, and the 8 staging
 // registers.  Same arithmetic, same per-element order of operations as semiring_tile_kernel (bit-exact).
 //
@@ -18,7 +17,7 @@
 
 #include <type_traits>
 
-#include "ptx_sm100.cuh"
+#include "ptx_sm90.cuh"
 #include "semiring.cuh"
 #include "tma_host.cuh"
 
@@ -119,41 +118,12 @@ semiring_ring_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_co
             bf[u][4 + q] = b1.v[q];
           }
         }
-        if constexpr (std::is_same<T, float>::value && PackedOp<Map>::value) {
-          F32x2 bp[2][4];
 #pragma unroll
-          for (int u = 0; u < 2; ++u)
+        for (int i = 0; i < 8; ++i) {
 #pragma unroll
-            for (int p = 0; p < 4; ++p) bp[u][p] = pack_f32x2(bf[u][2 * p], bf[u][2 * p + 1]);
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const F32x2 a0 = pack_f32x2(a4[i][kp], a4[i][kp]), a1 = pack_f32x2(a4[i][kp + 1], a4[i][kp + 1]);
-#pragma unroll
-            for (int p = 0; p < 4; ++p) {
-              const F32x2 t0 = PackedOp<Map>::Apply2(a0, bp[0][p]), t1 = PackedOp<Map>::Apply2(a1, bp[1][p]);
-              constexpr bool contractable =
-                  std::is_same<Map, Product<float>>::value && std::is_same<Reduce, Sum<float>>::value;
-              if constexpr (PackedOp<Reduce>::value && !contractable) {
-                const F32x2 r = PackedOp<Reduce>::Apply2(
-                    PackedOp<Reduce>::Apply2(pack_f32x2(acc[i][2 * p], acc[i][2 * p + 1]), t0), t1);
-                unpack_f32x2(r, acc[i][2 * p], acc[i][2 * p + 1]);
-              } else {
-                float t0l, t0h, t1l, t1h;
-                unpack_f32x2(t0, t0l, t0h);
-                unpack_f32x2(t1, t1l, t1h);
-                acc[i][2 * p] = Reduce::Apply(Reduce::Apply(acc[i][2 * p], t0l), t1l);
-                acc[i][2 * p + 1] = Reduce::Apply(Reduce::Apply(acc[i][2 * p + 1], t0h), t1h);
-              }
-            }
-          }
-        } else {
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              acc[i][j] = Reduce::Apply(Reduce::Apply(acc[i][j], Map::Apply(a4[i][kp], bf[0][j])),
-                                        Map::Apply(a4[i][kp + 1], bf[1][j]));
-            }
+          for (int j = 0; j < 8; ++j) {
+            acc[i][j] = Reduce::Apply(Reduce::Apply(acc[i][j], Map::Apply(a4[i][kp], bf[0][j])),
+                                      Map::Apply(a4[i][kp + 1], bf[1][j]));
           }
         }
       }

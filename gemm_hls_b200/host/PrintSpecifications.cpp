@@ -1,11 +1,11 @@
 // PrintSpecifications N K M [<SM clock MHz>]
 // Counterpart of the reference's specification printer (src/PrintSpecifications.cpp): pure
-// arithmetic on the build configuration, no device needed.  For the B200 kernels it reports the
+// arithmetic on the build configuration, no device needed.  For the H100 kernels it reports the
 // operation count, the kernel family this configuration dispatches to, that family's pipe-rate
 // model, whole-wave runtime estimates, and the reference's communication-volume model
 //   Q = N*M*(1 + K/T_N + K/T_M) elements            (src/PrintSpecifications.cpp:72-78)
 // evaluated twice: with the CTA tile (bytes through L2) and with the patch of C that the
-// co-running tiles share through L2 (bytes from HBM; profiles/r01_tile_sweep_half32768.csv).
+// co-running tiles share through L2 (bytes from HBM).
 #include <algorithm>
 #include <cmath>
 #include <iomanip>
@@ -22,21 +22,20 @@ struct KernelModel {
 };
 
 KernelModel ModelFor(std::string const &family, mmhost::Shape const &s) {
-  if (family == "tcgen05_f16") return {family, 2.0 * 4096, 256, 256, 2};   // UMMA 256x256x16 per 128 clk, CTA pair
-  if (family == "tcgen05_tf32") return {family, 2.0 * 2048, 256, 256, 2};  // UMMA 256x256x8  per 128 clk, CTA pair
-  if (family == "tcgen05_i8") return {family, 2.0 * 8192, 256, 256, 2};    // UMMA 256x256x32 per 128 clk, CTA pair
+  // wgmma, dense, per SM and clock: 2048 f16 / 1024 tf32 / 4096 8-bit multiply-adds; 256 x 256 tiles per CTA cluster
+  if (family == "wgmma_f16") return {family, 2.0 * 2048, 256, 256, 2};
+  if (family == "wgmma_tf32") return {family, 2.0 * 1024, 256, 256, 2};
+  if (family == "wgmma_i8") return {family, 2.0 * 4096, 256, 256, 2};
   if (family == "dmma_f64") {
-    // DMMA: 64 FMA / clk / SM; 128-row tiles, or 64-row tiles when those fill the last wave better
+    // DMMA: 128 FMA / clk / SM; 128-row tiles, or 64-row tiles when those fill the last wave better
     // (the launcher's rule, csrc/gemm_dmma.cu: the half-height tile has to win by more than 5 %)
     const double cols = (s.m + 127) / 128;
-    const double full = std::ceil(((s.n + 127) / 128) * cols / 148.0), half = 0.5 * 1.05 * std::ceil(((s.n + 63) / 64) * cols / 148.0);
-    return {family, 2.0 * 64, half < full ? 64u : 128u, 128, 1};
+    const double full = std::ceil(((s.n + 127) / 128) * cols / 132.0), half = 0.5 * 1.05 * std::ceil(((s.n + 63) / 64) * cols / 132.0);
+    return {family, 2.0 * 128, half < full ? 64u : 128u, 128, 1};
   }
-  // CUDA cores, one warp instruction per scheduler and clock (DESIGN.md 3.3): float (Add, Min|Max) issues
-  // 1 FADD2 + 1 FMNMX3 per two element-steps (128 steps/clk/SM), everything else is modelled at 1.5 slots
-  const bool packed_minmax = kDataTypeCode == MM_DTYPE_FLOAT && kMapOpCode == MM_OP_ADD &&
-                             (kReduceOpCode == MM_OP_MIN || kReduceOpCode == MM_OP_MAX) && !(kKernelFlags & MM_FLAG_EXACT);
-  return {family, 2.0 * (packed_minmax ? 128 : 85), 128, 128, 1};
+  // CUDA cores, one warp instruction per scheduler and clock (DESIGN.md 3.3): one Map and one Reduce
+  // instruction per element-step, 64 steps / clk / SM
+  return {family, 2.0 * 64, 128, 128, 1};
 }
 
 template <typename T>
@@ -58,8 +57,8 @@ int main(int argc, char **argv) {
   }
   mmhost::Shape s;
   const int next = mmhost::ReadShape(argv, 1, &s);
-  const double mhz = next < argc ? std::stod(argv[next]) : 1965.0;  // B200 clocks.max.sm
-  constexpr unsigned kSMs = 148;
+  const double mhz = next < argc ? std::stod(argv[next]) : 1980.0;  // H100 SXM clocks.max.sm
+  constexpr unsigned kSMs = 132;
 
   const KernelModel model = ModelFor(mm_kernel_path(kDataTypeCode, kMapOpCode, kReduceOpCode, kKernelFlags), s);
   const double ops = 2.0 * s.n * static_cast<double>(s.k) * s.m;

@@ -2,8 +2,8 @@
 // Drop-in for the reference's device launcher (host/RunHardware.cpp): same argument grammar, same
 // stdout sentences (the performance line is what scripts/build_manager.py:601-602 parses), same
 // exit codes.  Device work goes through Device.h (Context / Buffer / Kernel over the C-ABI).
-//   hw      the B200 selected by $MM_DEVICE (default 0)
-//   hw_emu  accepted for compatibility; there is no emulation target, it runs on the B200 as well
+//   hw      the H100 selected by $MM_DEVICE (default 0)
+//   hw_emu  accepted for compatibility; there is no emulation target, it runs on the H100 as well
 //   MM_NUM_GPUS=G (> 1)  C row-blocks over G GPUs inside libmm_b200.so (mm_multi_*): every GPU uploads 1/G of
 //                        B, the slices are gathered GPU-to-GPU over NVLink once, no per-step collective
 //   MM_POWER_METER=1  NVML power sampling every 10 ms while the kernel is repeated for >= 2 s, then
@@ -84,7 +84,7 @@ void RunSingle(mmhost::Problem &problem, bool verify) {
                                    c_device, shape.n, shape.k, shape.m);
   std::cout << "Executing kernel...\n" << std::flush;
   if (EnvironmentInt("MM_POWER_METER", 0) != 0) {
-    // A B200 kernel lasts milliseconds and NVML refreshes its reading every ~100 ms: repeat the
+    // A GPU kernel lasts milliseconds and NVML refreshes its reading every ~100 ms: repeat the
     // launch for at least two seconds under the meter and report the last run's time.
     mm::PowerMeter meter(10, static_cast<unsigned>(EnvironmentInt("MM_DEVICE", 0)));  // 10 ms, as the reference
     double device_seconds = 0, total = 0;

@@ -1,6 +1,6 @@
 // TestSimulation N K M
 // Drop-in for the reference's software test (test/TestSimulation.cpp): same arguments, same two
-// progress lines, same verdict sentence, same exit codes.  The "simulation" is the real B200 path
+// progress lines, same verdict sentence, same exit codes.  The "simulation" is the real H100 path
 // behind the same extern "C" MatrixMultiplicationKernel(a, b, c, n, k, m) call on host pointers.
 #include <stdexcept>
 

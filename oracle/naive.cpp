@@ -4,7 +4,7 @@
 // tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl
 // reference legs may load this; the product library (libmm_b200.so) never does.
 //
-// What is restated (reference file:line, all under /root/reference):
+// What is restated (reference file:line, all in the reference checkout):
 //   * Naive<OperatorMap, OperatorReduce>        include/Utility.h:18-42
 //       acc = OperatorReduce::identity(); for k: acc = Reduce(acc, Map(a, b));
 //       row-major A (N x K; K x N iff MM_TRANSPOSED_A, Utility.h:31-35),

@@ -1,6 +1,6 @@
 // TEST INFRASTRUCTURE ONLY.  Compiled by oracle/build.py once per
 // (MM_DATA_TYPE, MM_MAP_OP, MM_REDUCE_OP[, MM_TRANSPOSED_A]) against the
-// REFERENCE'S OWN headers where they lie under /root/reference (with the vendor
+// REFERENCE'S OWN headers where they lie in the reference checkout (with the vendor
 // headers the reference does not ship replaced by oracle/shim/), into
 // oracle/_ref/libref_naive_<cfg>.so.  The function body that runs is the
 // reference's Naive<> template, include/Utility.h:18-42, instantiated with the

@@ -1,13 +1,13 @@
 #!/bin/bash
 # Build the three host executables (TestSimulation, RunHardware, PrintSpecifications) with g++ against the
-# in-tree libmm_b200.so, without CMake (the GPU box receives sources + the .so, not a CMake build tree).
+# in-tree libmm_b200.so, without CMake.
 #   usage: bash scripts/build_host.sh [outdir] [float|double|half|int|...] [Multiply|Add|...] [Add|Min|...]
 #   MM_STATIC_SIZES="N K M" in the environment builds the MM_DYNAMIC_SIZES=OFF flavour (sizes fixed at
 #   compile time, executables take no N K M arguments), as the reference's CMake option does.
 #   MM_HOST_EXACT=1 / MM_HOST_HALF_TENSOR=1 = the CMake options -DMM_EXACT=ON / -DMM_HALF_TENSOR=ON.
 # MM_NUM_GPUS=G at run time splits the call over G GPUs inside libmm_b200.so (no NCCL needed).
 set -e
-R=${GRAFT_REPO_ROOT:-$(cd "$(dirname "$0")/.." && pwd)}
+R=$(cd "$(dirname "$0")/.." && pwd)
 OUT=${1:-/tmp/hostbuild}; TYPE=${2:-float}; MAP=${3:-Multiply}; RED=${4:-Add}
 mkdir -p "$OUT"
 read -r SN SK SM <<< "${MM_STATIC_SIZES:-512 512 512}"

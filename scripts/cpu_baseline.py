@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""CPU baseline of the reference's own path, timed on THIS host's cores (run it on the GPU box):
+"""CPU baseline of the reference's own path, timed on THIS host's cores (run it on the GPU machine):
   * the reference's Naive<> (include/Utility.h:18-42, compiled in place into oracle/_ref), single
     thread as written, at 256^3 / 1024^3 / 2048^3 (sampled rows at 2048^3) per configuration;
   * the reference's full TestSimulation (thread-per-stage software simulation of the FPGA kernel,

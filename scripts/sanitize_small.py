@@ -12,16 +12,16 @@ import oracle as O  # noqa: E402
 
 # (name, dtype, map, reduce, flags, (n, k, m)[, tuning])
 CASES = [
-    ("tcgen05_tf32", G.FLOAT, G.MULTIPLY, G.ADD, 0, (257, 48, 272)),
-    ("tcgen05_tf32 multi-tile", G.FLOAT, G.MULTIPLY, G.ADD, 0, (600, 80, 528)),
-    ("tcgen05_tf32 direct stores", G.FLOAT, G.MULTIPLY, G.ADD, 0, (257, 48, 272), dict(tma_store=0)),
-    ("tcgen05_tf32 overlapped B", G.FLOAT, G.MULTIPLY, G.ADD, 0, (257, 48, 528), dict(b_overlap=1)),
-    ("tcgen05_tf32 K-major B, 1 CTA, 128 cols", G.FLOAT, G.MULTIPLY, G.ADD, 0, (257, 48, 272), dict(b_mn=0, cta_group=1, block_n=128)),
-    ("tcgen05_i8", G.UINT8, G.MULTIPLY, G.ADD, 0, (257, 192, 320)),
-    ("tcgen05_i8 TA, 1 CTA", G.UINT8, G.MULTIPLY, G.ADD, G.FLAG_TRANSPOSED_A, (130, 64, 192), dict(cta_group=1)),
-    ("tcgen05_tf32 TA", G.FLOAT, G.MULTIPLY, G.ADD, G.FLAG_TRANSPOSED_A, (130, 64, 192)),
-    ("tcgen05_tf32x3", G.FLOAT, G.MULTIPLY, G.ADD, G.FLAG_TF32X3, (129, 48, 272)),
-    ("tcgen05_f16", G.HALF, G.MULTIPLY, G.ADD, 0, (257, 96, 288)),
+    ("wgmma_tf32", G.FLOAT, G.MULTIPLY, G.ADD, 0, (257, 48, 272)),
+    ("wgmma_tf32 multi-tile", G.FLOAT, G.MULTIPLY, G.ADD, 0, (600, 80, 528)),
+    ("wgmma_tf32 direct stores", G.FLOAT, G.MULTIPLY, G.ADD, 0, (257, 48, 272), dict(tma_store=0)),
+    ("wgmma_tf32 overlapped B", G.FLOAT, G.MULTIPLY, G.ADD, 0, (257, 48, 528), dict(b_overlap=1)),
+    ("wgmma_tf32 K-major B, 1 CTA, 128 cols", G.FLOAT, G.MULTIPLY, G.ADD, 0, (257, 48, 272), dict(b_mn=0, cta_group=1, block_n=128)),
+    ("wgmma_i8", G.UINT8, G.MULTIPLY, G.ADD, 0, (257, 192, 320)),
+    ("wgmma_i8 TA, 1 CTA", G.UINT8, G.MULTIPLY, G.ADD, G.FLAG_TRANSPOSED_A, (130, 64, 192), dict(cta_group=1)),
+    ("wgmma_tf32 TA", G.FLOAT, G.MULTIPLY, G.ADD, G.FLAG_TRANSPOSED_A, (130, 64, 192)),
+    ("wgmma_tf32x3", G.FLOAT, G.MULTIPLY, G.ADD, G.FLAG_TF32X3, (129, 48, 272)),
+    ("wgmma_f16", G.HALF, G.MULTIPLY, G.ADD, 0, (257, 96, 288)),
     ("dmma_f64", G.DOUBLE, G.MULTIPLY, G.ADD, 0, (130, 24, 136)),
     ("dmma_f64 TA", G.DOUBLE, G.MULTIPLY, G.ADD, G.FLAG_TRANSPOSED_A, (130, 24, 136)),
     ("dmma_f64 3 stages wrap", G.DOUBLE, G.MULTIPLY, G.ADD, 0, (70, 200, 264)),

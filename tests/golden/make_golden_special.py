@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Generate tests/golden/golden_special.json from the REFERENCE'S OWN Naive<> (include/Utility.h:18-42) on inputs the
 reference's recipe never produces: mixed signs, NaN / -0 / +0 / infinities, full-range bytes
-(tests/golden/special_inputs.py).  Authoring container only (needs /root/reference for oracle/_ref):
+(tests/golden/special_inputs.py).  Needs a reference checkout ($MM_REFERENCE_DIR) for oracle/_ref:
     python oracle/build.py && python tests/golden/make_golden_special.py
 """
 import hashlib
@@ -20,7 +20,7 @@ import special_inputs as S  # noqa: E402
 
 CASES = [
     # (dtype, map, reduce, input kind, seed, (n, k, m))
-    (O.UINT8, O.MULTIPLY, O.ADD, "bytes", 41, (513, 576, 576)),      # tcgen05 kind::i8: the modulo-256 wrap-around
+    (O.UINT8, O.MULTIPLY, O.ADD, "bytes", 41, (513, 576, 576)),      # 8-bit tensor cores: the modulo-256 wrap-around
     (O.UINT8, O.MULTIPLY, O.ADD, "bytes", 42, (129, 128, 192)),
     (O.FLOAT, O.ADD, O.MIN, "signed", 51, (257, 192, 144)),          # default flags (FMNMX) territory: no NaN, no zeros
     (O.FLOAT, O.ADD, O.MAX, "signed", 52, (65, 32, 48)),

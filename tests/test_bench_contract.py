@@ -1,6 +1,6 @@
 """bench.py's driver contract, as far as it can be exercised without a GPU: the reference arm
 (`--impl reference`: the reference's own Naive<> on the host cores) prints one JSON line with the agreed
-keys, non-zero ranks of a torchrun launch stay silent, and the B200 arm refuses to run without a device
+keys, non-zero ranks of a torchrun launch stay silent, and the GPU arm refuses to run without a device
 (no CPU fallback on the product path)."""
 import json
 import os
@@ -60,7 +60,7 @@ def test_b200_arm_has_no_cpu_fallback(mm):
 
 
 def test_cpu_baseline_object_of_the_b200_arm(oracle):
-    """The helper the B200 arm calls with host copies of its device inputs (no GPU needed to run it)."""
+    """The helper the GPU arm calls with host copies of its device inputs (no GPU needed to run it)."""
     import numpy as np
     sys.path.insert(0, ROOT)
     import bench

@@ -29,7 +29,7 @@ def _launch(mm, ctx, torch, dt, mp, rd, a, b, c, flags=0):
 
 
 def test_float_16384_cubed_properties(mm, oracle):
-    """BASELINE config 2: float 16384^3 on the tcgen05 path."""
+    """BASELINE config 2: float 16384^3 on the tensor-core path."""
     torch = pytest.importorskip("torch")
     n = k = m = 16384
     a, b, c = _device_problem(torch, torch.float32, n, k, m)

@@ -43,24 +43,24 @@ def _field(text, label):
 def test_print_specifications_float(host_float):
     r = _run(os.path.join(host_float, "PrintSpecifications"), 16384, 16384, 16384)
     assert r.returncode == 0, r.stderr
-    assert "float (Multiply, Add)" in r.stdout and "tcgen05_tf32" in r.stdout
+    assert "float (Multiply, Add)" in r.stdout and "wgmma_tf32" in r.stdout
     assert _field(r.stdout, "Number of operations:") == pytest.approx(2.0 * 16384 ** 3, rel=1e-5)
-    # 148 SMs x 4096 flop/clk x 1965 MHz
-    assert _field(r.stdout, "Ideal performance:") == pytest.approx(148 * 4096 * 1965e-3, rel=1e-4)
+    # 132 SMs x 2048 tf32 flop/clk x 1980 MHz
+    assert _field(r.stdout, "Ideal performance:") == pytest.approx(132 * 2048 * 1980e-3, rel=1e-4)
     assert _field(r.stdout, "Algorithmic bytes:") == pytest.approx(3 * 4 * 16384 ** 2, rel=1e-5)
     # the reference's I/O model with the CTA-pair tile as memory tile: N*M*(1 + K/256 + K/256) elements
     assert _field(r.stdout, "Communication volume:") == pytest.approx(16384.0 ** 2 * (1 + 64 + 64), rel=1e-5)
     slower = _run(os.path.join(host_float, "PrintSpecifications"), 16384, 16384, 16384, 1000)
-    assert _field(slower.stdout, "Ideal performance:") == pytest.approx(148 * 4096 * 1000e-3, rel=1e-4)
+    assert _field(slower.stdout, "Ideal performance:") == pytest.approx(132 * 2048 * 1000e-3, rel=1e-4)
 
 
 def test_print_specifications_uint8_uses_the_integer_tensor_model(mm, tmp_path):
     out = _build(tmp_path, "uint8_t")
     r = _run(os.path.join(out, "PrintSpecifications"), 16384, 16384, 16384)
     assert r.returncode == 0, r.stderr
-    assert "uint8_t (Multiply, Add)" in r.stdout and "tcgen05_i8" in r.stdout
-    # kind::i8: 148 SMs x 16384 op/clk x 1965 MHz (twice the 16-bit rate)
-    assert _field(r.stdout, "Ideal performance:") == pytest.approx(148 * 16384 * 1965e-3, rel=1e-4)
+    assert "uint8_t (Multiply, Add)" in r.stdout and "wgmma_i8" in r.stdout
+    # 8-bit wgmma: 132 SMs x 8192 op/clk x 1980 MHz (twice the 16-bit rate)
+    assert _field(r.stdout, "Ideal performance:") == pytest.approx(132 * 8192 * 1980e-3, rel=1e-4)
 
 
 def test_usage_and_shape_errors_follow_the_reference(host_float):
@@ -79,16 +79,16 @@ def test_usage_and_shape_errors_follow_the_reference(host_float):
 def test_double_model_picks_the_half_height_tile_for_short_row_blocks(mm, tmp_path):
     out = _build(tmp_path, "double")
     full = _run(os.path.join(out, "PrintSpecifications"), 8192, 8192, 8192).stdout
-    assert "dmma_f64" in full and "Compute tiles: 128x128 per CTA" in full and "28 waves" in full
-    block = _run(os.path.join(out, "PrintSpecifications"), 1024, 8192, 8192).stdout  # one GPU's share of the 8-GPU split
-    assert "Compute tiles: 64x128 per CTA" in block and "7 waves" in block
+    assert "dmma_f64" in full and "Compute tiles: 128x128 per CTA" in full and "32 waves" in full
+    block = _run(os.path.join(out, "PrintSpecifications"), 640, 8192, 8192).stdout  # 320 full tiles = 2.4 waves on 132 SMs
+    assert "Compute tiles: 64x128 per CTA" in block and "5 waves" in block
 
 
 def test_semiring_configuration_reports_the_cuda_core_family(mm, tmp_path):
     out = _build(tmp_path, "float", "Add", "Min")
     text = _run(os.path.join(out, "PrintSpecifications"), 8192, 8192, 8192).stdout
     assert "float (Add, Min)" in text and "semiring_simt" in text
-    assert _field(text, "Ideal performance:") == pytest.approx(148 * 256 * 1965e-3, rel=1e-4)
+    assert _field(text, "Ideal performance:") == pytest.approx(132 * 128 * 1980e-3, rel=1e-4)
 
 
 def test_static_size_build_takes_no_shape_arguments(mm, tmp_path):

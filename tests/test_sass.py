@@ -1,5 +1,5 @@
 """Static checks on the machine code of the built kernels (cuobjdump on the objects of
-gemm_hls_b200/build/, no GPU needed): the Blackwell-native instructions each path claims are there, and —
+gemm_hls_b200/build/, no GPU needed): the Hopper (sm_90a) instructions each path claims are there, and —
 the part that protects bit-exactness — ptxas has not contracted a multiply and an add into an FMA anywhere in
 the float / double / half semiring kernels (Naive<> rounds after the Map and again after the Reduce)."""
 import os
@@ -46,18 +46,19 @@ def _register_sources(instruction):
     return sum(1 for o in operands if re.match(r"^[-|~]*R\d+", o))
 
 
-def test_tensor_core_gemm_is_tcgen05_with_tma(mm):
-    funcs = {k: v for k, v in _functions("gemm_tcgen05.o").items() if "gemm_tcgen05_kernel" in k}
+def test_tensor_core_gemm_is_wgmma_with_tma(mm):
+    funcs = {k: v for k, v in _functions("gemm_tcgen05.o").items() if "gemm_wgmma_kernel" in k}
     assert funcs
     for name, ops in funcs.items():
-        assert _count(ops, "UTCHMMA") + _count(ops, "UTCIMMA") > 0, name   # tcgen05.mma (kind::tf32/f16 | kind::i8)
+        assert _count(ops, "HGMMA") + _count(ops, "IGMMA") > 0, name   # wgmma.mma_async (tf32 / f16 | u8)
         assert _count(ops, "UTMALDG") > 0, name          # cp.async.bulk.tensor loads
         assert _count(ops, "UTMASTG") > 0, name          # cp.async.bulk.tensor stores (the epilogue)
-        assert _count(ops, "LDTM") > 0, name             # tcgen05.ld (epilogue reads TMEM)
-        assert _count(ops, "HMMA") == 0 and _count(ops, "HGMMA") == 0, name   # no legacy tensor path
-    assert any(_count(ops, "UTCHMMA.2CTA") > 0 for ops in funcs.values())     # cta_group::2 variant exists
-    assert any(_count(ops, "UTCIMMA.2CTA") > 0 for ops in funcs.values())     # uint8_t on kind::i8, CTA pairs
-    assert len(funcs) == 24                               # {tf32, f16, i8} x {1, 2 CTAs} x {128, 256 columns} x {MN-, K-major B}
+        assert _count(ops, "HMMA") == 0 and _count(ops, "IMMA") == 0, name    # no warp-level mma.sync path
+        assert _count(ops, "LDL") == 0 and _count(ops, "STL") == 0, name      # accumulators stay in registers
+    assert sum(_count(ops, "HGMMA.64x256x8.F32.TF32") > 0 for ops in funcs.values()) == 2   # float, 1 and 2 CTAs
+    assert any(_count(ops, "IGMMA.64x256x32.U8.U8") > 0 for ops in funcs.values())          # uint8_t, exact s32
+    assert sum(_count(ops, "UTMALDG.2D.MULTICAST") > 0 for ops in funcs.values()) == 6      # cluster variants share B
+    assert len(funcs) == 12                               # {tf32, f16, u8} x {1, 2 CTAs} x {128, 256 columns}
 
 
 def test_double_gemm_is_dmma_fed_by_tma_without_ldgsts(mm):
@@ -88,16 +89,16 @@ def _semiring(obj, mp, rd, kernel="semiring_tile_kernel"):
     return out[0][1]
 
 
-def test_packed_float_paths(mm):
+def test_float_semiring_inner_loops(mm):
+    """One Map and one Reduce instruction per element and k step: 8 x 8 elements x 16 k per unrolled tile."""
     addmin = _semiring("semiring_f32_1.o", "Sum", "MinFast")
-    assert _count(addmin, "FADD2") == 512 and _count(addmin, "FMNMX3") == 512     # per 16-k tile: 1 + 1 per two steps
-    assert _count(addmin, "FADD") == _count(addmin, "FADD2")                       # no scalar FADD left
+    assert _count(addmin, "FADD") == 1024 and _count(addmin, "FMNMX") == 1024
     assert _count(addmin, "UTMALDG") > 0                                           # B tile staged by TMA
     ring = _semiring("semiring_f32_1.o", "Sum", "MinFast", kernel="semiring_ring_kernel")  # the default for 4-byte types
-    assert _count(ring, "FADD2") == 512 and _count(ring, "FMNMX3") == 512 and _count(ring, "FADD") == 512
+    assert _count(ring, "FADD") == 1024 and _count(ring, "FMNMX") == 1024
     assert _count(ring, "UTMALDG") >= 2 and _count(ring, "LDG") == 0 and _count(ring, "BAR") <= 2   # both tiles by TMA, no barrier in the loop
     exact = _semiring("semiring_f32_0.o", "Product", "Sum")
-    assert _count(exact, "FMUL2") == 512 and _count(exact, "FADD") - _count(exact, "FADD2") == 1024
+    assert _count(exact, "FMUL") == 1024 and _count(exact, "FADD") == 1024 and _count(exact, "FFMA") == 0
 
 
 @pytest.mark.parametrize("suffix", ["f32", "f64", "f16"])

@@ -55,7 +55,7 @@ def test_half_host_programs_take_the_reference_exact_branch(mm, tmp_path):
 
 
 def test_half_tensor_core_build_verifies_with_fp32_accumulation(mm, tmp_path):
-    """-DMM_HALF_TENSOR=ON: half on tcgen05 (FP32 accumulate); the host check uses an FP32-accumulated reference
+    """-DMM_HALF_TENSOR=ON: half on the tensor cores (FP32 accumulate); the host check uses an FP32-accumulated reference
     and the 1e-3 criterion (INTEGRATION.md section 3 states the deviation from the reference's half-in-half sum)."""
     out = _build(tmp_path, "half", MM_HOST_HALF_TENSOR="1")
     r = _run(os.path.join(out, "TestSimulation"), 513, 544, 544)
