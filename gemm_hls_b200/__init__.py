@@ -25,6 +25,7 @@ HALF, FLOAT, DOUBLE, INT32, UINT32, UINT8 = range(6)
 MULTIPLY, ADD, MIN, MAX, AND = range(5)
 # flags
 FLAG_NONE, FLAG_TRANSPOSED_A, FLAG_EXACT, FLAG_TF32X3 = 0, 1, 2, 4
+FLAG_BATCH_SHARED_A, FLAG_BATCH_SHARED_B = 8, 16   # batched calls: every problem reads the same A / B
 
 NP_DTYPE = {HALF: np.float16, FLOAT: np.float32, DOUBLE: np.float64,
             INT32: np.int32, UINT32: np.uint32, UINT8: np.uint8}
@@ -47,6 +48,7 @@ EXPORTS = ["mm_last_error", "mm_version", "mm_dtype_size", "mm_memory_width", "m
            "mm_copy_to_host", "mm_kernel_execute", "mm_kernel_enqueue", "mm_kernel_launch_count",
            "mm_kernel_path", "mm_gemm_host", "mm_context_set_profiling", "mm_context_profile_read",
            "mm_context_set_tuning", "mm_context_get_tuning", "mm_context_reserve",
+           "mm_kernel_enqueue_batched", "mm_context_reserve_batched",
            "mm_multi_create", "mm_multi_destroy", "mm_multi_device_count", "mm_multi_context",
            "mm_multi_peer_access", "mm_multi_partition", "mm_multi_gemm_host", "mm_multi_upload", "mm_multi_execute",
            "mm_multi_download"]
@@ -92,6 +94,8 @@ def lib():
         L.mm_context_set_tuning.argtypes = [vp, i, i]
         L.mm_context_get_tuning.argtypes = [vp, i, ctypes.POINTER(i)]
         L.mm_context_reserve.argtypes = [vp, i, i, u, u, u]
+        L.mm_kernel_enqueue_batched.argtypes = [vp, i, i, i, i, vp, vp, vp, u, u, u, u, vp]
+        L.mm_context_reserve_batched.argtypes = [vp, i, i, u, u, u, u]
         L.mm_multi_create.argtypes = [i, ctypes.POINTER(i), ctypes.POINTER(vp)]
         L.mm_multi_destroy.argtypes = [vp]
         L.mm_multi_device_count.argtypes = [vp]
@@ -179,6 +183,12 @@ class Context:
         _check(lib().mm_kernel_enqueue(self._h, dtype, map_op, reduce_op, flags, a_dev, b_dev, c_dev,
                                        n, k, m, ctypes.c_void_p(stream) if stream else None))
 
+    def enqueue_batched(self, dtype, map_op, reduce_op, a_dev, b_dev, c_dev, n, k, m, batch, flags=0, stream=None):
+        """`batch` packed problems (A at a + i*n*k, B at b + i*k*m unless FLAG_BATCH_SHARED_A / _B, C at
+        c + i*n*m elements) in one asynchronous launch sequence; each C equals its single enqueue bit for bit."""
+        _check(lib().mm_kernel_enqueue_batched(self._h, dtype, map_op, reduce_op, flags, a_dev, b_dev, c_dev,
+                                               n, k, m, batch, ctypes.c_void_p(stream) if stream else None))
+
     def set_tuning(self, **knobs):
         """mm_context_set_tuning by name, e.g. ctx.set_tuning(cta_group=1, stages=4)."""
         for name, value in knobs.items():
@@ -191,6 +201,9 @@ class Context:
 
     def reserve(self, dtype, n, k, m, flags=0):
         _check(lib().mm_context_reserve(self._h, dtype, flags, n, k, m))
+
+    def reserve_batched(self, dtype, n, k, m, batch, flags=0):
+        _check(lib().mm_context_reserve_batched(self._h, dtype, flags, n, k, m, batch))
 
     def set_profiling(self, enable=True):
         _check(lib().mm_context_set_profiling(self._h, int(enable)))

@@ -185,10 +185,36 @@ mm::GemmArgs make_args(mm_context *ctx, const void *a, const void *b, void *c, u
   return g;
 }
 
+// The problems of a batched call (mm_kernel_enqueue_batched); the single-problem entries pass batch = 1,
+// for which the MM_FLAG_BATCH_SHARED_* flags change nothing.
+mm::GemmBatch make_batch(unsigned batch, int flags) {
+  mm::GemmBatch bt;
+  bt.count = batch;
+  bt.shared_a = (flags & MM_FLAG_BATCH_SHARED_A) != 0;
+  bt.shared_b = (flags & MM_FLAG_BATCH_SHARED_B) != 0;
+  return bt;
+}
+
+// Rules of a batched call on top of check_args: batch in [1, 65535] (the kernels index problems by
+// gridDim.z, at most 65535), and the stacked extents batch * N, K, M below 2^31 (TMA coordinates are
+// signed 32-bit).
+int check_batch(unsigned batch, unsigned n, unsigned k, unsigned m) {
+  if (batch == 0) return fail(MM_ERR_INVALID, "batch must be positive");
+  if (batch > 65535) {
+    return fail(MM_ERR_UNSUPPORTED, "batch (" + std::to_string(batch) + ") must not exceed 65535");
+  }
+  const uint64_t limit = uint64_t(1) << 31;
+  if (uint64_t(batch) * n >= limit || uint64_t(batch) * k >= limit || uint64_t(batch) * m >= limit) {
+    return fail(MM_ERR_UNSUPPORTED, "batch * N, batch * K and batch * M must be below 2^31");
+  }
+  return MM_OK;
+}
+
 int enqueue_locked(mm_context *ctx, int dtype, int map_op, int reduce_op, int flags, const void *a,
                    const void *b, void *c, unsigned n, unsigned k, unsigned m, cudaStream_t stream,
-                   bool dry_run = false) {
+                   bool dry_run = false, unsigned batch = 1) {
   mm::GemmArgs g = make_args(ctx, a, b, c, n, k, m, flags, stream);
+  g.batch = make_batch(batch, flags);
   g.dry_run = dry_run;
   cudaStreamCaptureStatus capture = cudaStreamCaptureStatusNone;
   if (cudaStreamIsCapturing(stream, &capture) == cudaSuccess && capture != cudaStreamCaptureStatusNone) {
@@ -210,9 +236,10 @@ int enqueue_locked(mm_context *ctx, int dtype, int map_op, int reduce_op, int fl
   int rc_launch = MM_OK;
   switch (select_path(dtype, map_op, reduce_op, flags, n, k)) {
     case kPathTcgen05: {
-      const size_t need = mm::tcgen05_scratch_bytes(dtype, n, k, m, flags, ctx->tuning);
+      const size_t need = mm::tcgen05_scratch_bytes(dtype, n, k, m, flags, ctx->tuning, g.batch);
       if (need > ctx->scratch.bytes && capture != cudaStreamCaptureStatusNone) {
-        return fail(MM_ERR_INVALID, "the scratch cannot grow during stream capture: call mm_context_reserve() first");
+        return fail(MM_ERR_INVALID, batch > 1 ? "the scratch cannot grow during stream capture: call mm_context_reserve_batched() first"
+                                              : "the scratch cannot grow during stream capture: call mm_context_reserve() first");
       }
       int rc = ensure(ctx, ctx->scratch, need, ctx->captured);
       if (rc != MM_OK) return rc;
@@ -628,7 +655,7 @@ extern "C" {
 
 const char *mm_last_error(void) { return mm::g_last_error.c_str(); }
 
-int mm_version(void) { return 200; }
+int mm_version(void) { return 201; }
 
 size_t mm_dtype_size(int dtype) {
   switch (dtype) {
@@ -711,6 +738,20 @@ int mm_context_reserve(mm_context *ctx, int dtype, int flags, unsigned n, unsign
                 ctx->captured);
 }
 
+int mm_context_reserve_batched(mm_context *ctx, int dtype, int flags, unsigned n, unsigned k, unsigned m,
+                               unsigned batch) {
+  if (!ctx) return fail(MM_ERR_INVALID, "null context");
+  if (!valid_dtype(dtype)) return fail(MM_ERR_INVALID, "unknown MM_DATA_TYPE code");
+  int rc = check_batch(batch, n, k, m);
+  if (rc != MM_OK) return rc;
+  std::lock_guard<std::mutex> lock(ctx->mutex);
+  MM_CUDA_TRY(cudaSetDevice(ctx->device));
+  if (dtype != MM_DTYPE_FLOAT && dtype != MM_DTYPE_HALF && dtype != MM_DTYPE_UINT8) return MM_OK;  // only the tcgen05 path keeps scratch
+  const int f = flags & ~MM_FLAG_EXACT;
+  return ensure(ctx, ctx->scratch, mm::tcgen05_scratch_bytes(dtype, n, k, m, f, ctx->tuning, make_batch(batch, f)),
+                ctx->captured);
+}
+
 int mm_buffer_alloc(mm_context *ctx, size_t bytes, void **device_ptr) {
   if (!ctx || !device_ptr) return fail(MM_ERR_INVALID, "null argument");
   *device_ptr = nullptr;
@@ -759,6 +800,21 @@ int mm_kernel_enqueue(mm_context *ctx, int dtype, int map_op, int reduce_op, int
   MM_CUDA_TRY(cudaSetDevice(ctx->device));
   cudaStream_t s = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ctx->stream;
   return enqueue_locked(ctx, dtype, map_op, reduce_op, flags, a, b, c, n, k, m, s);
+}
+
+int mm_kernel_enqueue_batched(mm_context *ctx, int dtype, int map_op, int reduce_op, int flags, const void *a,
+                              const void *b, void *c, unsigned n, unsigned k, unsigned m, unsigned batch,
+                              void *cuda_stream) {
+  if (!ctx) return fail(MM_ERR_INVALID, "null context");
+  int rc = check_args(dtype, map_op, reduce_op, a, b, c, n, k, m);
+  if (rc != MM_OK) return rc;
+  if ((rc = check_batch(batch, n, k, m)) != MM_OK) return rc;
+  // every problem of a packed batch starts 16-byte aligned: K * sizeof(T) and M * sizeof(T) are multiples of 64
+  if ((rc = check_device_alignment(a, b, c)) != MM_OK) return rc;
+  std::lock_guard<std::mutex> lock(ctx->mutex);
+  MM_CUDA_TRY(cudaSetDevice(ctx->device));
+  cudaStream_t s = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ctx->stream;
+  return enqueue_locked(ctx, dtype, map_op, reduce_op, flags, a, b, c, n, k, m, s, /*dry_run=*/false, batch);
 }
 
 int mm_kernel_execute(mm_context *ctx, int dtype, int map_op, int reduce_op, int flags,

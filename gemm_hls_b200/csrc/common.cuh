@@ -54,6 +54,16 @@ struct Tuning {
 Tuning default_tuning();                                  // capi.cu
 int tuning_validate(int knob, int value);                 // MM_OK or MM_ERR_INVALID (message set)
 
+// A batch of `count` same-shape problems (mm_kernel_enqueue_batched).  Problem i reads A at
+// a + i * N * K elements and B at b + i * K * M, unless the operand is shared (every problem reads
+// the first one), and writes C at c + i * N * M.  A single call is a batch of one.
+struct GemmBatch {
+  unsigned count = 1;
+  bool shared_a = false, shared_b = false;
+  unsigned a_copies() const { return shared_a ? 1u : count; }  // distinct A (B) operands of the batch
+  unsigned b_copies() const { return shared_b ? 1u : count; }
+};
+
 struct GemmArgs {
   const void *a;
   const void *b;
@@ -62,6 +72,7 @@ struct GemmArgs {
   int flags;
   cudaStream_t stream;
   const Tuning *tuning = nullptr;  // never null on a real launch (capi.cu fills it from the context)
+  GemmBatch batch;
   // Second stream + fork/join events of the context: B's operand preparation runs there, overlapped
   // with the GEMM that consumes it panel by panel (gemm_tcgen05.cu).  Null = no overlap.
   cudaStream_t side_stream = nullptr;
@@ -84,8 +95,11 @@ int launch_semiring(int dtype, int map_op, int reduce_op, const GemmArgs &args);
 // The context's scratch holds, in this order: [B operand copy][A operand copy][counters].
 //   B operand copy: the transposed M x K copy wgmma reads K-major, rounded to TF32 for float.
 //   A operand copy: float = A rounded to TF32; any type with MM_FLAG_TRANSPOSED_A = A transposed.
-size_t tcgen05_scratch_bytes(int dtype, unsigned n, unsigned k, unsigned m, int flags, const Tuning &t);
-size_t tcgen05_bt_bytes(int dtype, unsigned k, unsigned m, int flags, const Tuning &t);  // = offset of the A copy
+// A batch keeps one copy per distinct operand (GemmBatch::a_copies / b_copies), packed.
+size_t tcgen05_scratch_bytes(int dtype, unsigned n, unsigned k, unsigned m, int flags, const Tuning &t,
+                             const GemmBatch &batch = GemmBatch{});
+size_t tcgen05_bt_bytes(int dtype, unsigned k, unsigned m, int flags, const Tuning &t,
+                        unsigned b_copies = 1);  // = offset of the A copy
 int launch_tcgen05(int dtype, const GemmArgs &args, void *scratch, size_t scratch_bytes);
 // How the kernel consumes B for this configuration.
 bool tcgen05_b_mn(int dtype, int flags, const Tuning &t);      // MN-major (row-major K x M array) vs K-major copy
@@ -113,8 +127,10 @@ Tcgen05Counters tcgen05_counters(void *scratch, size_t scratch_bytes);
 // it is read in place).  With `ready` non-null the pass runs panel by panel (BLOCK_N columns of B at
 // a time, in the order the GEMM's rasterisation consumes them) as a co-resident persistent kernel and
 // publishes each panel through ready[panel]; *ready_target receives the count that means "complete".
+// `copies` packed K x M problems of B are prepared into `copies` packed M x K copies (K-major path only).
 int tcgen05_prepare_b(int dtype, const BSource &src, void *bt, unsigned k, unsigned m, int flags, const Tuning &t,
-                      const void **b_op, unsigned int *ready, unsigned *ready_target, cudaStream_t stream);
+                      const void **b_op, unsigned int *ready, unsigned *ready_target, cudaStream_t stream,
+                      unsigned copies = 1);
 // Fork / join wrapper around tcgen05_prepare_b for the launchers: decides whether the preparation
 // overlaps the GEMM (float rounding, or any gather of peer slices, with the MN-major B path and a side
 // stream), zeroes the panel counters in stream order, runs the pass on `side` — ENQUEUED BEFORE the
@@ -129,14 +145,15 @@ struct PreparedB {
 };
 int tcgen05_prepare_b_async(int dtype, const BSource &src, void *local_b, void *scratch, size_t scratch_bytes,
                             unsigned k, unsigned m, int flags, const Tuning &t, cudaStream_t stream, cudaStream_t side,
-                            cudaEvent_t ev_fork, cudaEvent_t ev_join, PreparedB *out);
+                            cudaEvent_t ev_fork, cudaEvent_t ev_join, PreparedB *out, unsigned copies = 1);
+// `copies` packed problems of `rows` rows each.
 int tcgen05_prepare_a(int dtype, const void *a, void *aprep, unsigned rows, unsigned k, int flags, const Tuning &t,
-                      const void **a_op, cudaStream_t stream);
+                      const void **a_op, cudaStream_t stream, unsigned copies = 1);
 // `tile_sync`: device counter for the kernel's soft wave barrier, or null.  `b_ready` non-null: the
 // producer waits for b_ready[column tile] >= b_ready_target before it fetches a tile's B panel.
 int tcgen05_gemm(int dtype, const void *a_op, const void *b_op, void *c, unsigned rows, unsigned k, unsigned m,
                  int flags, const Tuning &t, unsigned int *tile_sync, const unsigned int *b_ready,
-                 unsigned b_ready_target, cudaStream_t stream);
+                 unsigned b_ready_target, cudaStream_t stream, const GemmBatch &batch = GemmBatch{});
 constexpr size_t kTcgen05TailBytes = 256 + 64 * 1024;  // [panel counters, 64 KiB][wave-barrier counter, 256 B]
 // Generic gather of row-sliced B into one local array (identity transform): what the multi-GPU path
 // uses for the kernel families that read B as is (double, semirings, half).

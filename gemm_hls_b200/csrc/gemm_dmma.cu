@@ -54,10 +54,15 @@ __device__ __forceinline__ void dmma_m8n8k4(double &c0, double &c1, double a, do
 // Every half-warp LDS.64 then reads sixteen distinct 8-byte words of one 128-byte bank row.
 constexpr int TMA_WM = 2, TMA_WN = 4;
 
+// Batch: blockIdx.z = problem.  B (K x M) and A stored K x N can be read past K (BK = 32, K % 8 == 0),
+// so their maps are 3-D {columns, K, problems} and zero-fill per problem; row-major A is a 2-D map with
+// the problems stacked along the rows (reading past N only feeds rows of C that are never stored).
+// a_step / b_step: 1 = packed operands, 0 = every problem reads problem 0's.
 template <bool TRANSPOSED_A, int BM>
 __global__ void __launch_bounds__((TMA_WM * TMA_WN + 1) * 32, 1)
 gemm_dmma_tma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
-                     double *__restrict__ C, unsigned size_n, unsigned size_k, unsigned size_m) {
+                     double *__restrict__ C, unsigned size_n, unsigned size_k, unsigned size_m, unsigned a_step,
+                     unsigned b_step) {
   constexpr int WM = TMA_WM, WN = TMA_WN, NCW = WM * WN;
   constexpr int MI = BM / (WM * 8), NJ = BN / (WN * 8);
   constexpr int WROWS = BM / WM;  // rows of C per warp
@@ -84,6 +89,7 @@ gemm_dmma_tma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_con
 
   if (warp == NCW) {
     if (lane != 0) return;
+    const int a_prob = int(blockIdx.z * a_step), b_prob = int(blockIdx.z * b_step);
     for (unsigned kt = 0; kt < k_tiles; ++kt) {
       const int stage = kt % STAGES;
       if (kt >= STAGES) mbar_wait(empty0 + 8 * stage, ((kt / STAGES) - 1) & 1);
@@ -91,20 +97,22 @@ gemm_dmma_tma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_con
       const int k0 = int(kt * BK);
       ptx::mbar_arrive_expect_tx(bar, STAGE_BYTES);
       if (!TRANSPOSED_A) {
+        const int a_row = a_prob * int(size_n) + int(row0);
 #pragma unroll
         for (int kh = 0; kh < BK / 16; ++kh)
-          ptx::tma_load_2d(as + kh * BM * 128, &map_a, bar, k0 + kh * 16, int(row0), ptx::L2_EVICT_NORMAL);
+          ptx::tma_load_2d(as + kh * BM * 128, &map_a, bar, k0 + kh * 16, a_row, ptx::L2_EVICT_NORMAL);
       } else {
 #pragma unroll
         for (int sl = 0; sl < BM / 16; ++sl)
-          ptx::tma_load_2d(as + sl * 4096, &map_a, bar, int(row0) + sl * 16, k0, ptx::L2_EVICT_NORMAL);
+          ptx::tma_load_3d(as + sl * 4096, &map_a, bar, int(row0) + sl * 16, k0, a_prob, ptx::L2_EVICT_NORMAL);
       }
 #pragma unroll
       for (int sl = 0; sl < BN / 16; ++sl)
-        ptx::tma_load_2d(bs + sl * 4096, &map_b, bar, int(col0) + sl * 16, k0, ptx::L2_EVICT_NORMAL);
+        ptx::tma_load_3d(bs + sl * 4096, &map_b, bar, int(col0) + sl * 16, k0, b_prob, ptx::L2_EVICT_NORMAL);
     }
     return;
   }
+  C += size_t(blockIdx.z) * size_n * size_m;
 
   const int wr = warp / WN, wc = warp % WN;
   const int g = lane / 4, q = lane % 4;
@@ -185,15 +193,18 @@ static int launch_dmma_tma(const GemmArgs &g) {
   MM_CUDA_TRY(cudaFuncSetAttribute(gemm_dmma_tma_kernel<true, BM>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(SMEM)));
   if (g.dry_run) return MM_OK;
   CUtensorMap map_a, map_b;
-  const int ra = ta ? encode_sw128_2d_f64(&map_a, g.a, g.k, g.n, BK) : encode_sw128_2d_f64(&map_a, g.a, g.n, g.k, BM);
-  const int rb = encode_sw128_2d_f64(&map_b, g.b, g.k, g.m, BK);
+  const unsigned na = g.batch.a_copies(), nb = g.batch.b_copies();
+  const int ra = ta ? encode_sw128_3d_f64(&map_a, g.a, g.k, g.n, na, BK)
+                    : encode_sw128_2d_f64(&map_a, g.a, uint64_t(na) * g.n, g.k, BM);
+  const int rb = encode_sw128_3d_f64(&map_b, g.b, g.k, g.m, nb, BK);
   if (ra != 0 || rb != 0) return fail(MM_ERR_CUDA, "cuTensorMapEncodeTiled failed for the f64 operands");
-  dim3 grid(ceil_div(g.m, BN), ceil_div(g.n, BM));
+  dim3 grid(ceil_div(g.m, BN), ceil_div(g.n, BM), g.batch.count);
   double *c = static_cast<double *>(g.c);
+  const unsigned a_step = g.batch.shared_a ? 0u : 1u, b_step = g.batch.shared_b ? 0u : 1u;
   if (ta) {
-    gemm_dmma_tma_kernel<true, BM><<<grid, THREADS, SMEM, g.stream>>>(map_a, map_b, c, g.n, g.k, g.m);
+    gemm_dmma_tma_kernel<true, BM><<<grid, THREADS, SMEM, g.stream>>>(map_a, map_b, c, g.n, g.k, g.m, a_step, b_step);
   } else {
-    gemm_dmma_tma_kernel<false, BM><<<grid, THREADS, SMEM, g.stream>>>(map_a, map_b, c, g.n, g.k, g.m);
+    gemm_dmma_tma_kernel<false, BM><<<grid, THREADS, SMEM, g.stream>>>(map_a, map_b, c, g.n, g.k, g.m, a_step, b_step);
   }
   MM_CUDA_TRY(cudaGetLastError());
   return MM_OK;
@@ -217,7 +228,9 @@ int launch_dmma(const GemmArgs &g) {
   int sms = 132, dev = 0;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  const double t128 = double(ceil_div(g.n, 128)) * ceil_div(g.m, BN), t64 = double(ceil_div(g.n, 64)) * ceil_div(g.m, BN);
+  // (tiles of the whole batch: its problems run side by side in one grid)
+  const double tiles_c = double(g.batch.count) * ceil_div(g.m, BN);
+  const double t128 = double(ceil_div(g.n, 128)) * tiles_c, t64 = double(ceil_div(g.n, 64)) * tiles_c;
   const double cost128 = std::ceil(t128 / sms), cost64 = 0.5 * 1.05 * std::ceil(t64 / sms);
   const int forced = g.tuning ? g.tuning->dmma_tile_rows() : 0;
   const bool use64 = forced == 64 || (forced != 128 && cost64 < cost128);

@@ -72,19 +72,23 @@ struct Geo {
 
 struct TileCoord {
   uint32_t r, c;
+  uint32_t prob;  // problem of a batched call
 };
 
 // Grouped rasterisation: RASTER_GROUP row-tiles sweep all column-tiles together so that the
 // concurrently running tiles share A row-panels and B column-panels through L2.  Column tiles are
-// visited in ascending order within a group.
+// visited in ascending order within a group.  In a batch the problem is the outermost index: the
+// tiles of problem i are tiles [i * tiles_r * tiles_c, (i + 1) * tiles_r * tiles_c), rasterised as above.
 __device__ __forceinline__ TileCoord tile_coord(uint32_t t, uint32_t tiles_r, uint32_t tiles_c,
                                                 uint32_t raster_group) {
+  const uint32_t prob = t / (tiles_r * tiles_c);
+  t -= prob * (tiles_r * tiles_c);
   const uint32_t per_group = raster_group * tiles_c;
   const uint32_t g = t / per_group;
   const uint32_t first = g * raster_group;
   const uint32_t gsize = min(raster_group, tiles_r - first);
   const uint32_t in = t - g * per_group;
-  return TileCoord{first + in % gsize, in / gsize};
+  return TileCoord{first + in % gsize, in / gsize, prob};
 }
 
 // ---- epilogue ------------------------------------------------------------------------------------
@@ -151,6 +155,10 @@ struct GemmParams {
   uint32_t raster_group;     // row tiles per rasterisation group
   uint32_t tma_store;        // 1: staged TMA-store epilogue, 0: direct stores
   uint32_t b_ready_target;   // see b_ready
+  // Batch: `batch` problems of rows x cols.  A and B are read through 2-D maps with the problems
+  // stacked along the row dimension: problem i starts at row i * a_prob_rows of A and
+  // i * b_prob_rows of B (0 = every problem reads the same operand).  C is a 3-D map {cols, rows, batch}.
+  uint32_t batch, a_prob_rows, b_prob_rows;
   uint64_t l2_policy;
   unsigned int *tile_sync;        // soft wave-barrier counter or null
   const unsigned int *b_ready;    // per column tile: preparation items finished, or null (B complete)
@@ -185,7 +193,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
 
   const uint32_t tiles_r = (rows + G::TILE_ROWS - 1) / G::TILE_ROWS;
   const uint32_t tiles_c = (cols + BN - 1) / BN;
-  const uint32_t num_tiles = tiles_r * tiles_c;
+  const uint32_t num_tiles = p.batch * tiles_r * tiles_c;
   const uint32_t num_kb = (p.k_bytes + BLOCK_K_BYTES - 1) / BLOCK_K_BYTES;
 
   if (threadIdx.x == 0) {
@@ -222,8 +230,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
           }
         }
         const TileCoord tc = tile_coord(t, tiles_r, tiles_c, p.raster_group);
-        const int32_t a_row = tc.r * G::TILE_ROWS + cta_rank * BLOCK_M;
-        const int32_t b_row = tc.c * BN + cta_rank * G::LOAD_N;
+        // Rows past the end of a problem belong to the next one: they only feed rows / columns of C
+        // that are never stored.  K is the inner dimension, so the K tail is zero-filled per row.
+        const int32_t a_row = tc.prob * p.a_prob_rows + tc.r * G::TILE_ROWS + cta_rank * BLOCK_M;
+        const int32_t b_row = tc.prob * p.b_prob_rows + tc.c * BN + cta_rank * G::LOAD_N;
         if (p.b_ready != nullptr && int32_t(tc.c) != ready_panel) {
           // B's preparation kernel was ENQUEUED before this kernel and needs no resource this kernel
           // holds, so it always makes progress; the bound only turns an impossible wait into a trap.
@@ -317,17 +327,19 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
             ptx::fence_proxy_async_smem();                        // generic-proxy smem writes -> TMA read
             __syncwarp();
             if (lane == 0) {
-              ptx::tma_store_2d(&tmap_c, buf, int32_t(col), int32_t(row0));  // clipped to rows x cols by the map
+              // clipped to rows x cols of this problem by the map
+              ptx::tma_store_3d(&tmap_c, buf, int32_t(col), int32_t(row0), int32_t(tc.prob));
               ptx::tma_store_commit();
             }
           }
         }
       } else {
+        TOut *Cp = C + size_t(tc.prob) * rows * cols;
 #pragma unroll
         for (int i = 0; i < 2; ++i) {
           const uint32_t row = row0 + r_in + 8 * i;
           if (row >= rows) continue;
-          typename P::T *crow = reinterpret_cast<typename P::T *>(C + size_t(row) * cols);
+          typename P::T *crow = reinterpret_cast<typename P::T *>(Cp + size_t(row) * cols);
 #pragma unroll
           for (int j = 0; j < BN / 8; ++j) {
             const uint32_t col = tc.c * BN + 8 * j + c_in;
@@ -440,7 +452,8 @@ __device__ __forceinline__ float prep_value<float, true>(float x) {
 }
 
 // dst[c][r] = f(src[r][c]) for src of shape src_rows x src_cols (row-major): 64 x 64 tiles through
-// shared memory so that both the reads and the writes are row-contiguous.
+// shared memory so that both the reads and the writes are row-contiguous.  blockIdx.z = problem of a
+// batch: packed sources, packed destinations.
 template <typename T, bool ROUND>
 __global__ void __launch_bounds__(256)
 transpose_prep_kernel(const T *__restrict__ src, T *__restrict__ dst, uint32_t src_rows,
@@ -448,6 +461,8 @@ transpose_prep_kernel(const T *__restrict__ src, T *__restrict__ dst, uint32_t s
   constexpr int TILE = 64;
   constexpr int PAD = (sizeof(T) >= 4) ? 1 : 2;
   __shared__ T tile[TILE][TILE + PAD];
+  src += size_t(blockIdx.z) * src_rows * src_cols;
+  dst += size_t(blockIdx.z) * src_rows * src_cols;
   const uint32_t c0 = blockIdx.x * TILE;
   const uint32_t r0 = blockIdx.y * TILE;
   const int x = threadIdx.x % TILE;
@@ -501,13 +516,16 @@ split3_rows_kernel(const float4 *__restrict__ src, float4 *__restrict__ dst, siz
 }
 
 // src (src_rows = K) x (src_cols) row-major -> dst[c][3K] with per-16-block [a | b | c] where
-// B_ORDER selects (hi, lo, hi) for the B operand and (hi, hi, lo) for a transposed A.
+// B_ORDER selects (hi, lo, hi) for the B operand and (hi, hi, lo) for a transposed A.  blockIdx.z =
+// problem of a batch, as in transpose_prep_kernel.
 template <bool B_ORDER>
 __global__ void __launch_bounds__(256)
 split3_transpose_kernel(const float *__restrict__ src, float *__restrict__ dst, uint32_t src_rows,
                         uint32_t src_cols) {
   constexpr int TILE = 64;
   __shared__ float tile[TILE][TILE + 1];
+  src += size_t(blockIdx.z) * src_rows * src_cols;
+  dst += size_t(blockIdx.z) * src_rows * src_cols * 3;
   const uint32_t c0 = blockIdx.x * TILE;
   const uint32_t r0 = blockIdx.y * TILE;
   const int x = threadIdx.x % TILE;
@@ -565,11 +583,25 @@ int make_operand_map(CUtensorMap *map, const void *base, int dtype, uint64_t row
                 CU_TENSOR_MAP_SWIZZLE_128B, "K-major operand");
 }
 
-// C (row-major rows x m) for the epilogue's TMA stores: 16 x 32 blocks, swizzle = row pitch of the block.
-int make_c_map(CUtensorMap *map, void *base, int dtype, uint64_t rows, uint64_t m) {
+// C (`batch` packed row-major rows x m matrices) for the epilogue's TMA stores: 16 x 32 blocks,
+// swizzle = row pitch of the block.  Three dimensions {m, rows, batch}, so that a block of a
+// problem whose last rows are partial is clipped at that problem's end, not the batch's.
+int make_c_map(CUtensorMap *map, void *base, int dtype, uint64_t rows, uint64_t m, uint64_t batch) {
   const uint32_t eb = elem_bytes(dtype);
-  return encode(map, tma_dtype(dtype), base, m, rows, m * eb, 32, EPI_ROWS,
-                eb == 4 ? CU_TENSOR_MAP_SWIZZLE_128B : (eb == 2 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B), "C");
+  EncodeTiledFn enc = get_encode_fn();
+  if (!enc) return fail(MM_ERR_CUDA, "cuTensorMapEncodeTiled entry point not available");
+  cuuint64_t gdim[3] = {m, rows, batch};
+  cuuint64_t gstride[2] = {m * eb, rows * m * eb};
+  cuuint32_t box[3] = {32, EPI_ROWS, 1};
+  cuuint32_t estr[3] = {1, 1, 1};
+  const CUtensorMapSwizzle swizzle =
+      eb == 4 ? CU_TENSOR_MAP_SWIZZLE_128B : (eb == 2 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B);
+  CUresult r = enc(map, tma_dtype(dtype), 3, base, gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle,
+                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    return fail(MM_ERR_CUDA, "cuTensorMapEncodeTiled (C) failed with CUresult " + std::to_string(int(r)));
+  }
+  return MM_OK;
 }
 
 int num_sms() {
@@ -582,8 +614,9 @@ int num_sms() {
 size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
 template <typename T, bool ROUND>
-void launch_transpose(const void *src, void *dst, uint32_t src_rows, uint32_t src_cols, cudaStream_t stream) {
-  dim3 grid((src_cols + 63) / 64, (src_rows + 63) / 64);
+void launch_transpose(const void *src, void *dst, uint32_t src_rows, uint32_t src_cols, cudaStream_t stream,
+                      unsigned copies) {
+  dim3 grid((src_cols + 63) / 64, (src_rows + 63) / 64, copies);
   transpose_prep_kernel<T, ROUND><<<grid, 256, 0, stream>>>(static_cast<const T *>(src), static_cast<T *>(dst),
                                                            src_rows, src_cols);
 }
@@ -628,17 +661,18 @@ bool tcgen05_b_in_place(int dtype, int flags, const Tuning &t) {
   return tcgen05_b_mn(dtype, flags, t) && (dtype == MM_DTYPE_HALF || dtype == MM_DTYPE_UINT8 || t.tf32_no_round());
 }
 
-size_t tcgen05_bt_bytes(int dtype, unsigned k, unsigned m, int flags, const Tuning &t) {
+size_t tcgen05_bt_bytes(int dtype, unsigned k, unsigned m, int flags, const Tuning &t, unsigned b_copies) {
   if (tcgen05_b_in_place(dtype, flags, t)) return 0;
   const size_t eb = elem_bytes(dtype);
-  return align_up(size_t(m) * k * eb * (split3(dtype, flags) ? 3 : 1), 1024);
+  return align_up(size_t(b_copies) * m * k * eb * (split3(dtype, flags) ? 3 : 1), 1024);
 }
 
-size_t tcgen05_scratch_bytes(int dtype, unsigned n, unsigned k, unsigned m, int flags, const Tuning &t) {
+size_t tcgen05_scratch_bytes(int dtype, unsigned n, unsigned k, unsigned m, int flags, const Tuning &t,
+                             const GemmBatch &batch) {
   const size_t eb = elem_bytes(dtype);
-  size_t bytes = TAIL_BYTES + tcgen05_bt_bytes(dtype, k, m, flags, t);  // counters (tail) + B copy
+  size_t bytes = TAIL_BYTES + tcgen05_bt_bytes(dtype, k, m, flags, t, batch.b_copies());  // counters (tail) + B copies
   if (dtype == MM_DTYPE_FLOAT || (flags & MM_FLAG_TRANSPOSED_A)) {
-    bytes += align_up(size_t(n) * k * eb * (split3(dtype, flags) ? 3 : 1), 1024);
+    bytes += align_up(size_t(batch.a_copies()) * n * k * eb * (split3(dtype, flags) ? 3 : 1), 1024);
   }
   return bytes;
 }
@@ -651,12 +685,14 @@ int gather_b_rows(const BSource &src, void *dst, size_t elem_bytes, unsigned k, 
 }
 
 int tcgen05_prepare_b(int dtype, const BSource &src, void *bt, unsigned k, unsigned m, int flags, const Tuning &t,
-                      const void **b_op, unsigned int *ready, unsigned *ready_target, cudaStream_t stream) {
+                      const void **b_op, unsigned int *ready, unsigned *ready_target, cudaStream_t stream,
+                      unsigned copies) {
   *b_op = bt;
   if (ready_target) *ready_target = 0;
   const bool parts = src.src != nullptr;
   const size_t eb = elem_bytes(dtype);
   if (tcgen05_b_mn(dtype, flags, t)) {
+    if (copies != 1) return fail(MM_ERR_UNSUPPORTED, "batched calls need the K-major B copy");
     const bool in_place = tcgen05_b_in_place(dtype, flags, t);
     if (in_place && !parts) {
       *b_op = src.b;  // nothing to prepare
@@ -697,18 +733,18 @@ int tcgen05_prepare_b(int dtype, const BSource &src, void *bt, unsigned k, unsig
   const void *b = src.b;
   if (parts) return fail(MM_ERR_UNSUPPORTED, "row-sliced B needs the MN-major B path (gather it first)");
   if (split3(dtype, flags)) {
-    dim3 grid((m + 63) / 64, (k + 63) / 64);
+    dim3 grid((m + 63) / 64, (k + 63) / 64, copies);
     split3_transpose_kernel<true><<<grid, 256, 0, stream>>>(static_cast<const float *>(b), static_cast<float *>(bt), k, m);
   } else if (dtype == MM_DTYPE_FLOAT) {
     if (t.tf32_no_round()) {
-      launch_transpose<float, false>(b, bt, k, m, stream);
+      launch_transpose<float, false>(b, bt, k, m, stream, copies);
     } else {
-      launch_transpose<float, true>(b, bt, k, m, stream);
+      launch_transpose<float, true>(b, bt, k, m, stream, copies);
     }
   } else if (dtype == MM_DTYPE_UINT8) {
-    launch_transpose<unsigned char, false>(b, bt, k, m, stream);
+    launch_transpose<unsigned char, false>(b, bt, k, m, stream, copies);
   } else {
-    launch_transpose<__half, false>(b, bt, k, m, stream);
+    launch_transpose<__half, false>(b, bt, k, m, stream, copies);
   }
   MM_CUDA_TRY(cudaGetLastError());
   return MM_OK;
@@ -716,43 +752,45 @@ int tcgen05_prepare_b(int dtype, const BSource &src, void *bt, unsigned k, unsig
 
 // `rows` rows of A -> the K-major A operand.  Row-major float A is rounded into `aprep`; row-major
 // half A is used in place; A stored K x N (`transposed`, leading dimension = rows, only whole
-// matrices) is transposed into `aprep`.  *a_op receives the operand pointer.
+// matrices) is transposed into `aprep`.  *a_op receives the operand pointer.  `copies` packed problems:
+// the row-wise passes run over copies * rows rows, the transposes take the problem from blockIdx.z.
 int tcgen05_prepare_a(int dtype, const void *a, void *aprep, unsigned rows, unsigned k, int flags, const Tuning &t,
-                      const void **a_op, cudaStream_t stream) {
+                      const void **a_op, cudaStream_t stream, unsigned copies) {
   const bool transposed = (flags & MM_FLAG_TRANSPOSED_A) != 0;
+  const size_t all_rows = size_t(copies) * rows;
   *a_op = a;
   if (split3(dtype, flags)) {
     if (transposed) {
-      dim3 grid((rows + 63) / 64, (k + 63) / 64);
+      dim3 grid((rows + 63) / 64, (k + 63) / 64, copies);
       split3_transpose_kernel<false><<<grid, 256, 0, stream>>>(static_cast<const float *>(a),
                                                               static_cast<float *>(aprep), k, rows);
     } else {
-      const size_t total4 = size_t(rows) * k / 4;
+      const size_t total4 = all_rows * k / 4;
       const int blocks = int(std::min<size_t>((total4 + 255) / 256, size_t(num_sms()) * 16));
       split3_rows_kernel<<<blocks, 256, 0, stream>>>(static_cast<const float4 *>(a),
-                                                    static_cast<float4 *>(aprep), rows, k);
+                                                    static_cast<float4 *>(aprep), all_rows, k);
     }
     *a_op = aprep;
   } else if (dtype == MM_DTYPE_FLOAT) {
     if (transposed) {
       if (t.tf32_no_round()) {
-        launch_transpose<float, false>(a, aprep, k, rows, stream);
+        launch_transpose<float, false>(a, aprep, k, rows, stream, copies);
       } else {
-        launch_transpose<float, true>(a, aprep, k, rows, stream);  // A stored K x N -> N x K
+        launch_transpose<float, true>(a, aprep, k, rows, stream, copies);  // A stored K x N -> N x K
       }
       *a_op = aprep;
     } else if (!t.tf32_no_round()) {
       MM_CUDA_TRY(cudaFuncSetAttribute(round_tf32_kernel, cudaFuncAttributePreferredSharedMemoryCarveout,
                                        cudaSharedmemCarveoutMaxShared));  // see tcgen05_prepare_b
-      const size_t count4 = size_t(rows) * k / 4;
+      const size_t count4 = all_rows * k / 4;
       const int blocks = int(std::min<size_t>((count4 + 255) / 256, size_t(num_sms()) * 16));
       round_tf32_kernel<<<blocks, 256, 0, stream>>>(static_cast<const float4 *>(a),
                                                    static_cast<float4 *>(aprep), count4);
       *a_op = aprep;
     }
   } else if (transposed) {
-    if (dtype == MM_DTYPE_UINT8) launch_transpose<unsigned char, false>(a, aprep, k, rows, stream);
-    else launch_transpose<__half, false>(a, aprep, k, rows, stream);
+    if (dtype == MM_DTYPE_UINT8) launch_transpose<unsigned char, false>(a, aprep, k, rows, stream, copies);
+    else launch_transpose<__half, false>(a, aprep, k, rows, stream, copies);
     *a_op = aprep;
   }
   MM_CUDA_TRY(cudaGetLastError());
@@ -782,7 +820,7 @@ int launch_gemm_variant(LaunchPlan plan) {
   if (plan.attributes_only) return MM_OK;
   plan.p.num_stages = uint32_t(stages);
   plan.p.raster_group = std::max<uint32_t>(1u, plan.p.raster_group / G::TILE_ROWS);  // rows -> row tiles
-  const uint32_t tiles = ceil_div(plan.p.rows, G::TILE_ROWS) * ceil_div(plan.p.cols, BN);
+  const uint32_t tiles = plan.p.batch * ceil_div(plan.p.rows, G::TILE_ROWS) * ceil_div(plan.p.cols, BN);
   const uint32_t groups = std::min<uint32_t>(tiles, uint32_t(num_sms()) / CG);
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(groups * CG);
@@ -815,26 +853,31 @@ int dispatch_variant(int cg, int bn, const LaunchPlan &plan) {
 
 int gemm_dispatch(int dtype, const void *a_op, const void *b_op, void *c, unsigned rows, unsigned k, unsigned m,
                   int flags, const Tuning &t, unsigned int *tile_sync, const unsigned int *b_ready,
-                  unsigned b_ready_target, bool attributes_only, cudaStream_t stream) {
+                  unsigned b_ready_target, bool attributes_only, cudaStream_t stream, const GemmBatch &batch) {
   if (split3(dtype, flags)) k *= 3;  // the operands carry [hi|hi|lo] x [hi|lo|hi] per 16-block of K
   const bool is_f32 = dtype == MM_DTYPE_FLOAT;
   const size_t eb = elem_bytes(dtype);
   const int cg = t.cta_group(), bn = t.block_n();
+  if (batch.count > 1 && b_ready != nullptr) return fail(MM_ERR_UNSUPPORTED, "batched calls need a complete B operand");
   CUtensorMap map_a, map_b, map_c;
   std::memset(&map_c, 0, sizeof(map_c));
   LaunchPlan plan{&map_a, &map_b, &map_c, c, {}, t.stages(), attributes_only, stream};
   if (!attributes_only) {
-    int rc = make_operand_map(&map_a, a_op, dtype, rows, k, BLOCK_M);
+    // the problems of a batch stacked along the rows (one copy when the operand is shared)
+    int rc = make_operand_map(&map_a, a_op, dtype, uint64_t(batch.a_copies()) * rows, k, BLOCK_M);
     if (rc != MM_OK) return rc;
-    rc = make_operand_map(&map_b, b_op, dtype, m, k, uint32_t(bn / cg));
+    rc = make_operand_map(&map_b, b_op, dtype, uint64_t(batch.b_copies()) * m, k, uint32_t(bn / cg));
     if (rc != MM_OK) return rc;
     if (t.tma_store()) {
-      rc = make_c_map(&map_c, c, dtype, rows, m);
+      rc = make_c_map(&map_c, c, dtype, rows, m, batch.count);
       if (rc != MM_OK) return rc;
     }
   }
   plan.p.rows = rows;
   plan.p.cols = m;
+  plan.p.batch = batch.count;
+  plan.p.a_prob_rows = batch.shared_a ? 0u : rows;
+  plan.p.b_prob_rows = batch.shared_b ? 0u : m;
   plan.p.k_bytes = uint32_t(size_t(k) * eb);
   plan.p.raster_group = uint32_t(std::max(1, t.raster_rows()));  // in rows here; per-variant tiles in the launcher
   plan.p.tma_store = t.tma_store() ? 1u : 0u;
@@ -852,16 +895,21 @@ int gemm_dispatch(int dtype, const void *a_op, const void *b_op, void *c, unsign
 // C[rows x m] = Aop[rows x k] * B on the tensor cores; `b_op` as returned by tcgen05_prepare_b.
 int tcgen05_gemm(int dtype, const void *a_op, const void *b_op, void *c, unsigned rows, unsigned k, unsigned m,
                  int flags, const Tuning &t, unsigned int *tile_sync, const unsigned int *b_ready,
-                 unsigned b_ready_target, cudaStream_t stream) {
-  return gemm_dispatch(dtype, a_op, b_op, c, rows, k, m, flags, t, tile_sync, b_ready, b_ready_target, false, stream);
+                 unsigned b_ready_target, cudaStream_t stream, const GemmBatch &batch) {
+  return gemm_dispatch(dtype, a_op, b_op, c, rows, k, m, flags, t, tile_sync, b_ready, b_ready_target, false, stream,
+                       batch);
 }
 
 int tcgen05_prepare_b_async(int dtype, const BSource &src, void *local_b, void *scratch, size_t scratch_bytes,
                             unsigned k, unsigned m, int flags, const Tuning &t, cudaStream_t stream, cudaStream_t side,
-                            cudaEvent_t ev_fork, cudaEvent_t ev_join, PreparedB *out) {
+                            cudaEvent_t ev_fork, cudaEvent_t ev_join, PreparedB *out, unsigned copies) {
   *out = PreparedB{};
   const bool in_place = tcgen05_b_in_place(dtype, flags, t);
   const bool parts = src.src != nullptr;
+  if (copies != 1) {
+    if (parts) return fail(MM_ERR_UNSUPPORTED, "batched calls take B from one array");
+    return tcgen05_prepare_b(dtype, src, scratch, k, m, flags, t, &out->b_op, nullptr, nullptr, stream, copies);
+  }
   if (parts && !tcgen05_b_mn(dtype, flags, t)) {
     // K-major copy requested (tuning / 3xTF32): assemble the slices first, then transpose locally
     int rc = gather_b_rows(src, local_b, elem_bytes(dtype), k, m, stream);
@@ -903,25 +951,27 @@ int launch_tcgen05(int dtype, const GemmArgs &g, void *scratch, size_t scratch_b
     MM_CUDA_TRY(cudaFuncGetAttributes(&attr, transpose_prep_kernel<__half, false>));
     MM_CUDA_TRY(cudaFuncGetAttributes(&attr, transpose_prep_kernel<unsigned char, false>));
     if (!get_encode_fn()) return fail(MM_ERR_CUDA, "cuTensorMapEncodeTiled entry point not available");
-    return gemm_dispatch(dtype, nullptr, nullptr, nullptr, g.n, g.k, g.m, g.flags, t, nullptr, nullptr, 0, true, g.stream);
+    return gemm_dispatch(dtype, nullptr, nullptr, nullptr, g.n, g.k, g.m, g.flags, t, nullptr, nullptr, 0, true, g.stream,
+                         g.batch);
   }
-  if (scratch_bytes < tcgen05_scratch_bytes(dtype, g.n, g.k, g.m, g.flags, t)) {
+  if (scratch_bytes < tcgen05_scratch_bytes(dtype, g.n, g.k, g.m, g.flags, t, g.batch)) {
     return fail(MM_ERR_INVALID, "tcgen05 scratch too small");
   }
   unsigned char *sp = static_cast<unsigned char *>(scratch);
-  void *aprep = sp + tcgen05_bt_bytes(dtype, g.k, g.m, g.flags, t);
+  void *aprep = sp + tcgen05_bt_bytes(dtype, g.k, g.m, g.flags, t, g.batch.b_copies());
   const Tcgen05Counters cnt = tcgen05_counters(scratch, scratch_bytes);
   BSource src;
   src.b = g.b;
   PreparedB pb;
   const void *a_op = nullptr;
+  // one preparation pass per operand for the whole batch; a shared operand is prepared once
   int rc = tcgen05_prepare_b_async(dtype, src, nullptr, scratch, scratch_bytes, g.k, g.m, g.flags, t, g.stream,
-                                   g.side_stream, g.ev_fork, g.ev_join, &pb);
-  if (rc == MM_OK) rc = tcgen05_prepare_a(dtype, g.a, aprep, g.n, g.k, g.flags, t, &a_op, g.stream);
+                                   g.side_stream, g.ev_fork, g.ev_join, &pb, g.batch.b_copies());
+  if (rc == MM_OK) rc = tcgen05_prepare_a(dtype, g.a, aprep, g.n, g.k, g.flags, t, &a_op, g.stream, g.batch.a_copies());
   if (rc == MM_OK && g.ev_prep_done) cudaEventRecord(g.ev_prep_done, g.stream);
   if (rc == MM_OK) {
     rc = tcgen05_gemm(dtype, a_op, pb.b_op, g.c, g.n, g.k, g.m, g.flags, t, cnt.tile_sync, pb.ready, pb.ready_target,
-                      g.stream);
+                      g.stream, g.batch);
   }
   if (pb.forked) cudaStreamWaitEvent(g.stream, g.ev_join, 0);  // join, on the error paths too
   return rc;

@@ -95,6 +95,22 @@ __device__ __forceinline__ void tma_store_2d(const void *tmap, uint32_t smem_src
                "r"(smem_src), "r"(c0), "r"(c1)
                : "memory");
 }
+// 3-D tile load / store: c2 = outermost coordinate (the problem of a batched call).
+__device__ __forceinline__ void tma_load_3d(uint32_t smem_dst, const void *tmap, uint32_t bar,
+                                            int32_t c0, int32_t c1, int32_t c2, uint64_t l2_policy) {
+  asm volatile(
+      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
+      " [%0], [%1, {%3, %4, %5}], [%2], %6;" ::"r"(smem_dst),
+      "l"(reinterpret_cast<uint64_t>(tmap)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "l"(l2_policy)
+      : "memory");
+}
+__device__ __forceinline__ void tma_store_3d(const void *tmap, uint32_t smem_src, int32_t c0, int32_t c1,
+                                             int32_t c2) {
+  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];" ::"l"(
+                   reinterpret_cast<uint64_t>(tmap)),
+               "r"(smem_src), "r"(c0), "r"(c1), "r"(c2)
+               : "memory");
+}
 __device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void tma_store_wait_read() {

@@ -9,11 +9,11 @@ namespace {
 template <typename T>
 int by_map(int map_op, int reduce_op, const GemmArgs &g, bool ta, bool ring) {
   switch (map_op) {
-    case MM_OP_MULTIPLY: return launch_semiring_for<T, MM_OP_MULTIPLY>(reduce_op, g.a, g.b, g.c, g.n, g.k, g.m, ta, ring, g.stream);
-    case MM_OP_ADD: return launch_semiring_for<T, MM_OP_ADD>(reduce_op, g.a, g.b, g.c, g.n, g.k, g.m, ta, ring, g.stream);
-    case MM_OP_MIN: return launch_semiring_for<T, MM_OP_MIN>(reduce_op, g.a, g.b, g.c, g.n, g.k, g.m, ta, ring, g.stream);
-    case MM_OP_MAX: return launch_semiring_for<T, MM_OP_MAX>(reduce_op, g.a, g.b, g.c, g.n, g.k, g.m, ta, ring, g.stream);
-    case MM_OP_AND: return launch_semiring_for<T, MM_OP_AND>(reduce_op, g.a, g.b, g.c, g.n, g.k, g.m, ta, ring, g.stream);
+    case MM_OP_MULTIPLY: return launch_semiring_for<T, MM_OP_MULTIPLY>(reduce_op, g.a, g.b, g.c, g.n, g.k, g.m, ta, ring, g.batch, g.stream);
+    case MM_OP_ADD: return launch_semiring_for<T, MM_OP_ADD>(reduce_op, g.a, g.b, g.c, g.n, g.k, g.m, ta, ring, g.batch, g.stream);
+    case MM_OP_MIN: return launch_semiring_for<T, MM_OP_MIN>(reduce_op, g.a, g.b, g.c, g.n, g.k, g.m, ta, ring, g.batch, g.stream);
+    case MM_OP_MAX: return launch_semiring_for<T, MM_OP_MAX>(reduce_op, g.a, g.b, g.c, g.n, g.k, g.m, ta, ring, g.batch, g.stream);
+    case MM_OP_AND: return launch_semiring_for<T, MM_OP_AND>(reduce_op, g.a, g.b, g.c, g.n, g.k, g.m, ta, ring, g.batch, g.stream);
   }
   return -1;
 }
@@ -21,8 +21,8 @@ int by_map(int map_op, int reduce_op, const GemmArgs &g, bool ta, bool ring) {
 // float only: the hardware min/max variants (internal operator codes)
 int by_map_float(int map_op, int reduce_op, const GemmArgs &g, bool ta, bool ring) {
   switch (map_op) {
-    case MM_OP_MIN_FAST: return launch_semiring_for<float, MM_OP_MIN_FAST>(reduce_op, g.a, g.b, g.c, g.n, g.k, g.m, ta, ring, g.stream);
-    case MM_OP_MAX_FAST: return launch_semiring_for<float, MM_OP_MAX_FAST>(reduce_op, g.a, g.b, g.c, g.n, g.k, g.m, ta, ring, g.stream);
+    case MM_OP_MIN_FAST: return launch_semiring_for<float, MM_OP_MIN_FAST>(reduce_op, g.a, g.b, g.c, g.n, g.k, g.m, ta, ring, g.batch, g.stream);
+    case MM_OP_MAX_FAST: return launch_semiring_for<float, MM_OP_MAX_FAST>(reduce_op, g.a, g.b, g.c, g.n, g.k, g.m, ta, ring, g.batch, g.stream);
   }
   return by_map<float>(map_op, reduce_op, g, ta, ring);
 }

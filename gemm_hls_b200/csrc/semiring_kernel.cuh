@@ -21,6 +21,10 @@
 // (cp.async.bulk.tensor + mbarrier complete_tx), the same mechanism the tensor-core path uses.
 // No warp-shuffle reduction is needed (or wanted): K is never split across lanes, which is what
 // keeps the reduction order — and therefore every rounding — identical to Naive<>.
+//
+// Batch: blockIdx.z = problem.  B's map holds the problems stacked along K (a tile never crosses a
+// problem: K % BK == 0); A and C take per-problem pointer offsets.  a_step / b_step: 1 = packed
+// operands, 0 = every problem reads problem 0's.
 #pragma once
 
 #include <cuda_runtime.h>
@@ -28,6 +32,7 @@
 #include <cstdint>
 #include <type_traits>
 
+#include "common.cuh"
 #include "ptx_sm90.cuh"
 #include "semiring.cuh"
 #include "tma_host.cuh"
@@ -77,10 +82,13 @@ template <typename T, class Map, class Reduce>
 __global__ void __launch_bounds__(256, (sizeof(T) == 4 || SemiringHalf2<T, Map, Reduce>::value) ? 2 : 1)
 semiring_tile_kernel(const T *__restrict__ A, const __grid_constant__ CUtensorMap tmap_b, T *__restrict__ C,
                      unsigned size_n, unsigned size_k, unsigned size_m,
-                     bool TRANSPOSED_A) {
+                     bool TRANSPOSED_A, unsigned a_step, unsigned b_step) {
   using Cfg = SemiringTile<T>;
   constexpr int BM = Cfg::BM, BN = Cfg::BN, BK = Cfg::BK, VEC = Cfg::VEC;
   constexpr int LDA = Cfg::LDA, LDB = Cfg::LDB;
+  A += size_t(blockIdx.z * a_step) * size_n * size_k;
+  C += size_t(blockIdx.z) * size_n * size_m;
+  const unsigned b_k0 = blockIdx.z * b_step * size_k;  // first row of this problem's B in the map
 
   extern __shared__ __align__(128) unsigned char smem_raw[];
   T *As = reinterpret_cast<T *>(smem_raw);                          // [2][BK][LDA]  (k-major: A transposed)
@@ -119,7 +127,7 @@ semiring_tile_kernel(const T *__restrict__ A, const __grid_constant__ CUtensorMa
   auto load_b_tma = [&](int buf, unsigned k0) {
     if (tid == 0) {
       ptx::mbar_arrive_expect_tx(bar0 + 8 * buf, uint32_t(Cfg::B_TILE_BYTES));
-      ptx::tma_load_2d(ptx::smem_u32(Bs + buf * BK * LDB), &tmap_b, bar0 + 8 * buf, int32_t(col0), int32_t(k0),
+      ptx::tma_load_2d(ptx::smem_u32(Bs + buf * BK * LDB), &tmap_b, bar0 + 8 * buf, int32_t(col0), int32_t(b_k0 + k0),
                        ptx::L2_EVICT_NORMAL);
     }
   };
@@ -272,29 +280,32 @@ namespace mm {
 
 template <typename T, class Map, class Reduce>
 int launch_semiring_typed(const void *a, const void *b, void *c, unsigned n, unsigned k, unsigned m,
-                          bool transposed_a, bool ring, cudaStream_t stream) {
+                          bool transposed_a, bool ring, const GemmBatch &batch, cudaStream_t stream) {
   using Cfg = SemiringTile<T>;
   if constexpr (sizeof(T) == 4) {
     // 4-byte types with A stored row-major take the ring variant (both tiles by TMA, no block-wide barrier:
     // 41.7 vs 39.9 TOp/s for float (Add, Min) at 8192^3); the tuning knob MM_TUNE_SEMIRING_RING = 0 keeps this kernel
     if (ring && !transposed_a && (a == nullptr || reinterpret_cast<uintptr_t>(a) % 16 == 0)) {
-      return launch_semiring_ring<T, Map, Reduce>(a, b, c, n, k, m, stream);
+      return launch_semiring_ring<T, Map, Reduce>(a, b, c, n, k, m, batch.count, batch.shared_a, batch.shared_b,
+                                                  stream);
     }
   }
   if (a == nullptr) {  // dry run: only make sure the kernel is loaded
     cudaFuncAttributes attr;
     return static_cast<int>(cudaFuncGetAttributes(&attr, semiring_tile_kernel<T, Map, Reduce>));
   }
-  dim3 grid((m + Cfg::BN - 1) / Cfg::BN, (n + Cfg::BM - 1) / Cfg::BM);
+  dim3 grid((m + Cfg::BN - 1) / Cfg::BN, (n + Cfg::BM - 1) / Cfg::BM, batch.count);
   dim3 block(Cfg::THREADS);
   const T *pa = static_cast<const T *>(a);
   T *pc = static_cast<T *>(c);
-  CUtensorMap tmap_b;  // B row-major K x M, box = BK rows x 128 columns
-  if (encode_plain_2d(&tmap_b, b, sizeof(T), k, m, Cfg::BK, Cfg::BN) != 0) {
+  // B row-major K x M (the problems of a batch stacked along K), box = BK rows x 128 columns
+  CUtensorMap tmap_b;
+  const uint64_t b_rows = uint64_t(batch.shared_b ? 1 : batch.count) * k;
+  if (encode_plain_2d(&tmap_b, b, sizeof(T), b_rows, m, Cfg::BK, Cfg::BN) != 0) {
     return static_cast<int>(cudaErrorInvalidValue);
   }
-  semiring_tile_kernel<T, Map, Reduce><<<grid, block, Cfg::SMEM_BYTES, stream>>>(pa, tmap_b, pc, n, k, m,
-                                                                                transposed_a);
+  semiring_tile_kernel<T, Map, Reduce><<<grid, block, Cfg::SMEM_BYTES, stream>>>(
+      pa, tmap_b, pc, n, k, m, transposed_a, batch.shared_a ? 0u : 1u, batch.shared_b ? 0u : 1u);
   return static_cast<int>(cudaGetLastError());
 }
 
@@ -303,18 +314,18 @@ int launch_semiring_typed(const void *a, const void *b, void *c, unsigned n, uns
 // build in parallel.
 template <typename T, int MAP_OP>
 int launch_semiring_for(int reduce_op, const void *a, const void *b, void *c, unsigned n, unsigned k,
-                        unsigned m, bool ta, bool ring, cudaStream_t stream);
+                        unsigned m, bool ta, bool ring, const GemmBatch &batch, cudaStream_t stream);
 
 #define MM_SEMIRING_CASE(REDOP)                                                                    \
   if (reduce_op == REDOP)                                                                          \
     return launch_semiring_typed<T, typename OpSelect<T, MAP_OP>::type,                            \
-                                 typename OpSelect<T, REDOP>::type>(a, b, c, n, k, m, ta, ring, stream);
+                                 typename OpSelect<T, REDOP>::type>(a, b, c, n, k, m, ta, ring, batch, stream);
 
 #define MM_INSTANTIATE_SEMIRING(TYPE, MAPOP)                                                       \
   template <>                                                                                      \
   int launch_semiring_for<TYPE, MAPOP>(int reduce_op, const void *a, const void *b, void *c,       \
                                        unsigned n, unsigned k, unsigned m, bool ta, bool ring,     \
-                                       cudaStream_t stream) {                                      \
+                                       const GemmBatch &batch, cudaStream_t stream) {          \
     using T = TYPE;                                                                                \
     constexpr int MAP_OP = MAPOP;                                                                  \
     MM_SEMIRING_CASE(MM_OP_MULTIPLY)                                                               \

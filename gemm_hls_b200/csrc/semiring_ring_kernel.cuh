@@ -38,10 +38,16 @@ struct SemiringRing {
 template <typename T, class Map, class Reduce>
 __global__ void __launch_bounds__(256, 2)
 semiring_ring_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-                     T *__restrict__ C, unsigned size_n, unsigned size_k, unsigned size_m) {
+                     T *__restrict__ C, unsigned size_n, unsigned size_k, unsigned size_m, unsigned a_step,
+                     unsigned b_step) {
   static_assert(sizeof(T) == 4, "ring variant: 4-byte element types");
   using Cfg = SemiringRing;
   constexpr int BM = Cfg::BM, BN = Cfg::BN, BK = Cfg::BK, STAGES = Cfg::STAGES;
+  // Batch (blockIdx.z = problem): both maps hold the problems stacked along their rows.  A tile of A
+  // may run past N into the next problem (those rows of C are never stored); a tile of B never crosses
+  // a problem (K % BK == 0).  a_step / b_step: 1 = packed operands, 0 = every problem reads problem 0's.
+  C += size_t(blockIdx.z) * size_n * size_m;
+  const unsigned a_row0 = blockIdx.z * a_step * size_n, b_k0 = blockIdx.z * b_step * size_k;
 
   extern __shared__ unsigned char smem_raw[];
   const uint32_t smem0 = (ptx::smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -71,8 +77,8 @@ semiring_ring_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_co
     if (kt >= STAGES) ptx::mbar_wait(empty0 + 8 * stage, ((kt / STAGES) - 1) & 1);
     const uint32_t as = smem0 + stage * Cfg::STAGE_BYTES, bs = as + Cfg::A_BYTES, bar = full0 + 8 * stage;
     ptx::mbar_arrive_expect_tx(bar, Cfg::STAGE_BYTES);
-    ptx::tma_load_2d(as, &tmap_a, bar, int32_t(kt * BK), int32_t(row0), ptx::L2_EVICT_NORMAL);
-    ptx::tma_load_2d(bs, &tmap_b, bar, int32_t(col0), int32_t(kt * BK), ptx::L2_EVICT_NORMAL);
+    ptx::tma_load_2d(as, &tmap_a, bar, int32_t(kt * BK), int32_t(a_row0 + row0), ptx::L2_EVICT_NORMAL);
+    ptx::tma_load_2d(bs, &tmap_b, bar, int32_t(col0), int32_t(b_k0 + kt * BK), ptx::L2_EVICT_NORMAL);
   };
   if (tid == 0) {
     for (unsigned kt = 0; kt < unsigned(Cfg::AHEAD) && kt < k_tiles; ++kt) load_tile(kt);
@@ -152,20 +158,23 @@ semiring_ring_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_co
 
 // Host side: nullptr A = dry run (load the kernel only).  Returns a cudaError_t value as int.
 template <typename T, class Map, class Reduce>
-int launch_semiring_ring(const void *a, const void *b, void *c, unsigned n, unsigned k, unsigned m,
-                         cudaStream_t stream) {
+int launch_semiring_ring(const void *a, const void *b, void *c, unsigned n, unsigned k, unsigned m, unsigned batch,
+                         bool shared_a, bool shared_b, cudaStream_t stream) {
   using Cfg = SemiringRing;
   auto kernel = semiring_ring_kernel<T, Map, Reduce>;
   cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(Cfg::SMEM_BYTES));
   if (e != cudaSuccess || a == nullptr) return static_cast<int>(e);
   CUtensorMap tmap_a, tmap_b;
-  // A row-major N x K: box = 128 rows x 16 k (64-byte rows); B row-major K x M: box = 16 k x 128 columns
-  if (encode_plain_2d(&tmap_a, a, sizeof(T), n, k, Cfg::BM, Cfg::BK) != 0 ||
-      encode_plain_2d(&tmap_b, b, sizeof(T), k, m, Cfg::BK, Cfg::BN) != 0) {
+  // A row-major N x K: box = 128 rows x 16 k (64-byte rows); B row-major K x M: box = 16 k x 128 columns;
+  // the problems of a batch stacked along the rows
+  const uint64_t a_rows = uint64_t(shared_a ? 1 : batch) * n, b_rows = uint64_t(shared_b ? 1 : batch) * k;
+  if (encode_plain_2d(&tmap_a, a, sizeof(T), a_rows, k, Cfg::BM, Cfg::BK) != 0 ||
+      encode_plain_2d(&tmap_b, b, sizeof(T), b_rows, m, Cfg::BK, Cfg::BN) != 0) {
     return static_cast<int>(cudaErrorInvalidValue);
   }
-  dim3 grid((m + Cfg::BN - 1) / Cfg::BN, (n + Cfg::BM - 1) / Cfg::BM);
-  kernel<<<grid, Cfg::THREADS, Cfg::SMEM_BYTES, stream>>>(tmap_a, tmap_b, static_cast<T *>(c), n, k, m);
+  dim3 grid((m + Cfg::BN - 1) / Cfg::BN, (n + Cfg::BM - 1) / Cfg::BM, batch);
+  kernel<<<grid, Cfg::THREADS, Cfg::SMEM_BYTES, stream>>>(tmap_a, tmap_b, static_cast<T *>(c), n, k, m,
+                                                          shared_a ? 0u : 1u, shared_b ? 0u : 1u);
   return static_cast<int>(cudaGetLastError());
 }
 

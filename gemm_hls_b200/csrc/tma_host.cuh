@@ -63,4 +63,19 @@ inline int encode_sw128_2d_f64(CUtensorMap *map, const void *base, uint64_t rows
                               CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE));
 }
 
+// `count` packed arrays of rows x cols as one 3-D tensor {cols, rows, count}: the same tiles, but
+// out-of-bounds reads past `rows` are zeros per array instead of the next array's first rows.
+inline int encode_sw128_3d_f64(CUtensorMap *map, const void *base, uint64_t rows, uint64_t cols, uint64_t count,
+                               uint32_t box_rows) {
+  EncodeTiledFn enc = get_encode_fn();
+  if (!enc) return -1;
+  cuuint64_t gdim[3] = {cols, rows, count};
+  cuuint64_t gstride[2] = {cols * 8, rows * cols * 8};
+  cuuint32_t box[3] = {16, box_rows, 1};
+  cuuint32_t estr[3] = {1, 1, 1};
+  return static_cast<int>(enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT64, 3, const_cast<void *>(base), gdim, gstride, box,
+                              estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                              CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE));
+}
+
 }  // namespace mm

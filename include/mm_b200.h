@@ -88,7 +88,11 @@ enum {
   /* float (Multiply, Add) on the tensor cores with the 3xTF32 split (hi*hi + hi*lo + lo*hi, each
    * operand split into two TF32 values): ~FP32 accuracy (about 1e-6 relative) at 1/3 of the TF32
    * rate.  Ignored for every other configuration. */
-  MM_FLAG_TF32X3 = 4
+  MM_FLAG_TF32X3 = 4,
+  /* Two flags, meaningful only in batched calls (mm_kernel_enqueue_batched).  The single-problem
+   * entries ignore them: a single call is a batch of one, so the statement holds trivially. */
+  MM_FLAG_BATCH_SHARED_A = 8,  /* every problem of the batch reads the same A */
+  MM_FLAG_BATCH_SHARED_B = 16  /* every problem of the batch reads the same B */
 };
 
 enum {
@@ -154,6 +158,22 @@ MM_API int mm_kernel_enqueue(mm_context *ctx, int dtype, int map_op, int reduce_
                       const void *a_device, const void *b_device, void *c_device, unsigned size_n,
                       unsigned size_k, unsigned size_m, void *cuda_stream);
 
+/* A batch of `batch` same-shape problems in one launch sequence, asynchronous like
+ * mm_kernel_enqueue().  Problem i (0 <= i < batch) reads A at a_device + i*N*K elements and B at
+ * b_device + i*K*M elements, unless MM_FLAG_BATCH_SHARED_A / _B says every problem reads the first
+ * one, and writes C at c_device + i*N*M elements.  Each matrix has the layout of a single call.
+ * The result of problem i is BIT-IDENTICAL to mm_kernel_enqueue() on that problem's A and B with the
+ * same flags and tuning, for every type, semiring, flag and tuning value.  The call launches the same
+ * kernels as one single call (mm_kernel_launch_count()), whatever the batch size: one preparation
+ * pass per operand over the whole batch (once for a shared operand) and one compute kernel.
+ * Validation as mm_kernel_enqueue(), plus: batch == 0 -> MM_ERR_INVALID; batch > 65535, or
+ * batch*N, batch*K or batch*M >= 2^31 -> MM_ERR_UNSUPPORTED.  Scratch grows with the number of
+ * distinct operands: size it with mm_context_reserve_batched() before a stream capture. */
+MM_API int mm_kernel_enqueue_batched(mm_context *ctx, int dtype, int map_op, int reduce_op, int flags,
+                                     const void *a_device, const void *b_device, void *c_device,
+                                     unsigned size_n, unsigned size_k, unsigned size_m,
+                                     unsigned batch, void *cuda_stream);
+
 /* Per-phase device timing of enqueued work, for roofline accounting.  With profiling on, every
  * mm_kernel_enqueue()/mm_kernel_execute() records CUDA events on the launching stream around
  * (i) the operand-preparation kernels and (ii) the main compute kernel.  mm_context_profile_read()
@@ -217,6 +237,10 @@ MM_API int mm_context_get_tuning(mm_context *ctx, int knob, int *value);
  * has seen a stream capture therefore keeps superseded allocations alive until it is destroyed. */
 MM_API int mm_context_reserve(mm_context *ctx, int dtype, int flags, unsigned size_n, unsigned size_k,
                               unsigned size_m);
+/* The same for mm_kernel_enqueue_batched() with these flags: one operand copy per problem, or one
+ * for an operand the flags mark as shared.  Batch rules as mm_kernel_enqueue_batched(). */
+MM_API int mm_context_reserve_batched(mm_context *ctx, int dtype, int flags, unsigned size_n,
+                                      unsigned size_k, unsigned size_m, unsigned batch);
 
 /* ---- multi-GPU: C row-blocks over the GPUs of one box (SURVEY.md section 8e) ------------------
  * The reference's API is ONE blocking call on host pointers (include/MatrixMultiplication.h:155-171)

@@ -50,6 +50,53 @@ for case in CASES:
     ok = O.verify(dt, c, ref) == -1 if G.kernel_path(dt, mp, rd, flags) == "semiring_simt" or dt != G.HALF else True
     print("%-42s %s" % (name, "ok" if ok else "MISMATCH"), flush=True)
     bad += 0 if ok else 1
+# batched calls (3 ragged problems, packed or shared operands): every problem equals its single call
+BATCHED = [
+    ("batched wgmma_tf32", G.FLOAT, G.MULTIPLY, G.ADD, 0, (257, 48, 272)),
+    ("batched wgmma_tf32 direct stores, shared B", G.FLOAT, G.MULTIPLY, G.ADD, G.FLAG_BATCH_SHARED_B, (129, 48, 272),
+     dict(tma_store=0)),
+    ("batched wgmma_f16 shared A", G.HALF, G.MULTIPLY, G.ADD, G.FLAG_BATCH_SHARED_A, (129, 96, 288)),
+    ("batched wgmma_i8 TA, 1 CTA", G.UINT8, G.MULTIPLY, G.ADD, G.FLAG_TRANSPOSED_A, (130, 64, 192), dict(cta_group=1)),
+    ("batched wgmma_tf32x3 TA", G.FLOAT, G.MULTIPLY, G.ADD, G.FLAG_TF32X3 | G.FLAG_TRANSPOSED_A, (130, 48, 144)),
+    ("batched dmma_f64", G.DOUBLE, G.MULTIPLY, G.ADD, 0, (130, 40, 136)),
+    ("batched dmma_f64 TA, shared B", G.DOUBLE, G.MULTIPLY, G.ADD, G.FLAG_TRANSPOSED_A | G.FLAG_BATCH_SHARED_B,
+     (130, 24, 136)),
+    ("batched semiring f32 addmin shared B", G.FLOAT, G.ADD, G.MIN, G.FLAG_BATCH_SHARED_B, (129, 48, 144)),
+    ("batched semiring i32 staged kernel", G.INT32, G.MULTIPLY, G.ADD, 0, (65, 32, 48), dict(semiring_ring=0)),
+    ("batched semiring f64 addmax TA", G.DOUBLE, G.ADD, G.MAX, G.FLAG_TRANSPOSED_A, (67, 16, 24)),
+]
+shared_flags = G.FLAG_BATCH_SHARED_A | G.FLAG_BATCH_SHARED_B
+for case in BATCHED:
+    name, dt, mp, rd, flags, (n, k, m) = case[:6]
+    tuning = case[6] if len(case) > 6 else {}
+    if only and only not in name:
+        continue
+    batch = 3
+    na = 1 if flags & G.FLAG_BATCH_SHARED_A else batch
+    nb = 1 if flags & G.FLAG_BATCH_SHARED_B else batch
+    data = [O.fill(dt, n, k, m, 40 + i) for i in range(batch)]
+    a = np.concatenate([d[0].reshape(-1) for d in data[:na]])
+    b = np.concatenate([d[1].reshape(-1) for d in data[:nb]])
+    if dt == G.HALF:
+        a = (a.astype(np.float32) * np.float32(0.25)).astype(np.float16)
+    with G.Context(0) as ctx:
+        ctx.set_tuning(**tuning)
+        da, db, dc = ctx.alloc(a.nbytes), ctx.alloc(b.nbytes), ctx.alloc(batch * n * m * a.itemsize)
+        ctx.copy_to_device(da, a)
+        ctx.copy_to_device(db, b)
+        ctx.enqueue_batched(dt, mp, rd, da, db, dc, n, k, m, batch, flags=flags)
+        c = np.empty((batch, n * m), dtype=a.dtype)
+        ctx.copy_to_host(c, dc)   # ordered after the enqueue on the context's stream
+        ok = True
+        for i in range(batch):
+            ai = a.reshape(na, -1)[0 if na == 1 else i]
+            bi = b.reshape(nb, -1)[0 if nb == 1 else i]
+            single = ctx.gemm_host(dt, mp, rd, ai, bi, n, k, m, flags=flags & ~shared_flags)[0]
+            ok = ok and single.tobytes() == c[i].tobytes()
+        for p in (da, db, dc):
+            ctx.free(p)
+    print("%-42s %s" % (name, "ok" if ok else "MISMATCH"), flush=True)
+    bad += 0 if ok else 1
 # the row-block split on one device listed twice: sliced upload of B, the gather kernel, host barriers
 if not only or "multi" in only:
     for dt, shape in ((G.FLOAT, (300, 128, 272)), (G.HALF, (257, 128, 288)), (G.DOUBLE, (130, 128, 136))):
