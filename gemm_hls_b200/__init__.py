@@ -19,18 +19,19 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 # MM_B200_LIB: A/B experiments load a variant build of the library; the product is the in-tree library
 LIB_PATH = os.environ.get("MM_B200_LIB") or os.path.join(HERE, "libmm_b200.so")
 
-# MM_DATA_TYPE codes
-HALF, FLOAT, DOUBLE, INT32, UINT32, UINT8 = range(6)
+# MM_DATA_TYPE codes (BFLOAT16 is a library-level extension: the reference has no such type)
+HALF, FLOAT, DOUBLE, INT32, UINT32, UINT8, BFLOAT16 = range(7)
 # MM_MAP_OP / MM_REDUCE_OP codes (hlslib::op functors)
 MULTIPLY, ADD, MIN, MAX, AND = range(5)
 # flags
 FLAG_NONE, FLAG_TRANSPOSED_A, FLAG_EXACT, FLAG_TF32X3 = 0, 1, 2, 4
 FLAG_BATCH_SHARED_A, FLAG_BATCH_SHARED_B = 8, 16   # batched calls: every problem reads the same A / B
 
+# numpy has no bfloat16: BFLOAT16 host arrays are its bit patterns (np.uint16, or ml_dtypes.bfloat16), taken by view
 NP_DTYPE = {HALF: np.float16, FLOAT: np.float32, DOUBLE: np.float64,
-            INT32: np.int32, UINT32: np.uint32, UINT8: np.uint8}
+            INT32: np.int32, UINT32: np.uint32, UINT8: np.uint8, BFLOAT16: np.uint16}
 DTYPE_FROM_NAME = {"half": HALF, "float": FLOAT, "double": DOUBLE, "int": INT32,
-                   "unsigned": UINT32, "unsigned int": UINT32, "uint8_t": UINT8}
+                   "unsigned": UINT32, "unsigned int": UINT32, "uint8_t": UINT8, "bfloat16": BFLOAT16}
 OP_FROM_NAME = {"Multiply": MULTIPLY, "Product": MULTIPLY, "Add": ADD, "Sum": ADD,
                 "Min": MIN, "Max": MAX, "And": AND}
 
@@ -279,9 +280,8 @@ class Multi:
         return _gemm_host(self._h, dtype, map_op, reduce_op, a, b, n, k, m, flags, out, fn=lib().mm_multi_gemm_host)
 
     def upload(self, dtype, a, b, n, k, m, flags=0):
-        npdt = NP_DTYPE[dtype]
-        a = np.ascontiguousarray(a, dtype=npdt).reshape(-1)
-        b = np.ascontiguousarray(b, dtype=npdt).reshape(-1)
+        a = _host_operand(dtype, a)
+        b = _host_operand(dtype, b)
         _check(lib().mm_multi_upload(self._h, dtype, flags, a.ctypes.data, b.ctypes.data, n, k, m))
 
     def execute(self, dtype, map_op, reduce_op, n, k, m, flags=0):
@@ -295,10 +295,25 @@ class Multi:
         return c
 
 
+def _host_operand(dtype, x):
+    """x as the flat contiguous host array the library reads.  BFLOAT16 takes any 2-byte array that is not a
+    floating-point numpy type (np.uint16 bit patterns, ml_dtypes.bfloat16) as it is: its bytes are the
+    bfloat16 values.  A float array would need a rounding the caller did not ask for, so it is refused."""
+    if dtype == BFLOAT16:
+        x = np.asarray(x)
+        if x.dtype.itemsize != 2 or x.dtype.kind == "f":
+            raise MMError(1, "BFLOAT16 takes bfloat16 bit patterns (np.uint16 or ml_dtypes.bfloat16 arrays), "
+                             "not %s: convert explicitly" % x.dtype)
+        return np.ascontiguousarray(x).reshape(-1)
+    return np.ascontiguousarray(x, dtype=NP_DTYPE.get(dtype)).reshape(-1)
+
+
 def _gemm_host(handle, dtype, map_op, reduce_op, a, b, n, k, m, flags, out, fn=None):
     npdt = NP_DTYPE.get(dtype)  # unknown codes are rejected by the library itself (MM_ERR_INVALID)
-    a = np.ascontiguousarray(a, dtype=npdt).reshape(-1)
-    b = np.ascontiguousarray(b, dtype=npdt).reshape(-1)
+    a = _host_operand(dtype, a)
+    b = _host_operand(dtype, b)
+    if dtype == BFLOAT16:
+        npdt = a.dtype  # C comes back with A's dtype
     if npdt is not None and (a.size != n * k or b.size != k * m):
         raise MMError(1, "A must hold n*k and B k*m elements")
     c = out if out is not None else np.empty((n, m), dtype=npdt if npdt is not None else a.dtype)

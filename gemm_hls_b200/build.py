@@ -21,10 +21,11 @@ ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 FLAGS = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden",
          "--expt-relaxed-constexpr"]
 
-SOURCES = ["capi.cu", "gemm_tcgen05.cu", "gemm_dmma.cu", "semiring_dispatch.cu"]
+SOURCES = ["capi.cu", "gemm_tcgen05.cu", "gemm_wgmma_bf16.cu", "gemm_dmma.cu", "semiring_dispatch.cu"]
 # semiring_inst.cu is compiled once per (type, map operator): (object suffix, C type)
 INST_TYPES = [("f16", "__half"), ("f32", "float"), ("f64", "double"), ("i32", "int"),
-              ("u32", "unsigned"), ("u8", "unsigned char")]
+              ("u32", "unsigned"), ("u8", "unsigned char"),
+              ("bf16", "__nv_bfloat16")]
 INST_MAPS = [0, 1, 2, 3, 4]  # MM_OP_MULTIPLY .. MM_OP_AND
 
 

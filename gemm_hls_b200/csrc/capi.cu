@@ -114,13 +114,18 @@ bool valid_op(int o) { return o >= 0 && o < MM_OP_COUNT; }
 
 enum Path { kPathTcgen05, kPathDmma, kPathSemiring };
 
+// The types the wgmma GEMM takes for (Multiply, Add).
+bool tensor_core_dtype(int d) {
+  return d == MM_DTYPE_FLOAT || d == MM_DTYPE_HALF || d == MM_DTYPE_BFLOAT16 || d == MM_DTYPE_UINT8;
+}
+
 // uint8_t on the integer tensor cores: products accumulate exactly in 32-bit integers while 255^2 * K < 2^31; the low byte
 // of the exact sum is the reference's modulo-256 arithmetic.  Longer K takes the CUDA-core kernel.
 constexpr unsigned kMaxKInt8Tensor = 33024;
 
 Path select_path(int dtype, int map_op, int reduce_op, int flags, unsigned n, unsigned k) {
   const bool dense = (map_op == MM_OP_MULTIPLY && reduce_op == MM_OP_ADD) && !(flags & MM_FLAG_EXACT);
-  if (dense && (dtype == MM_DTYPE_FLOAT || dtype == MM_DTYPE_HALF)) return kPathTcgen05;
+  if (dense && (dtype == MM_DTYPE_FLOAT || dtype == MM_DTYPE_HALF || dtype == MM_DTYPE_BFLOAT16)) return kPathTcgen05;
   if (dense && dtype == MM_DTYPE_UINT8 && k <= kMaxKInt8Tensor) return kPathTcgen05;
   if (dense && dtype == MM_DTYPE_DOUBLE) {
     // the DMMA kernel reads a transposed A through 16-byte boxes: needs an even N
@@ -655,7 +660,7 @@ extern "C" {
 
 const char *mm_last_error(void) { return mm::g_last_error.c_str(); }
 
-int mm_version(void) { return 201; }
+int mm_version(void) { return 202; }
 
 size_t mm_dtype_size(int dtype) {
   switch (dtype) {
@@ -665,6 +670,7 @@ size_t mm_dtype_size(int dtype) {
     case MM_DTYPE_INT32: return 4;
     case MM_DTYPE_UINT32: return 4;
     case MM_DTYPE_UINT8: return 1;
+    case MM_DTYPE_BFLOAT16: return 2;
   }
   return 0;
 }
@@ -733,7 +739,7 @@ int mm_context_reserve(mm_context *ctx, int dtype, int flags, unsigned n, unsign
   if (!valid_dtype(dtype)) return fail(MM_ERR_INVALID, "unknown MM_DATA_TYPE code");
   std::lock_guard<std::mutex> lock(ctx->mutex);
   MM_CUDA_TRY(cudaSetDevice(ctx->device));
-  if (dtype != MM_DTYPE_FLOAT && dtype != MM_DTYPE_HALF && dtype != MM_DTYPE_UINT8) return MM_OK;  // only the tcgen05 path keeps scratch
+  if (!tensor_core_dtype(dtype)) return MM_OK;  // only the tcgen05 path keeps scratch
   return ensure(ctx, ctx->scratch, mm::tcgen05_scratch_bytes(dtype, n, k, m, flags & ~MM_FLAG_EXACT, ctx->tuning),
                 ctx->captured);
 }
@@ -746,7 +752,7 @@ int mm_context_reserve_batched(mm_context *ctx, int dtype, int flags, unsigned n
   if (rc != MM_OK) return rc;
   std::lock_guard<std::mutex> lock(ctx->mutex);
   MM_CUDA_TRY(cudaSetDevice(ctx->device));
-  if (dtype != MM_DTYPE_FLOAT && dtype != MM_DTYPE_HALF && dtype != MM_DTYPE_UINT8) return MM_OK;  // only the tcgen05 path keeps scratch
+  if (!tensor_core_dtype(dtype)) return MM_OK;  // only the tcgen05 path keeps scratch
   const int f = flags & ~MM_FLAG_EXACT;
   return ensure(ctx, ctx->scratch, mm::tcgen05_scratch_bytes(dtype, n, k, m, f, ctx->tuning, make_batch(batch, f)),
                 ctx->captured);
@@ -893,7 +899,9 @@ int mm_kernel_launch_count(int dtype, int map_op, int reduce_op, int flags) {
 const char *mm_kernel_path(int dtype, int map_op, int reduce_op, int flags) {
   if (!valid_dtype(dtype) || !valid_op(map_op) || !valid_op(reduce_op)) return "invalid";
   switch (select_path(dtype, map_op, reduce_op, flags, 2, 64)) {
-    case kPathTcgen05: return dtype == MM_DTYPE_FLOAT ? "wgmma_tf32" : (dtype == MM_DTYPE_UINT8 ? "wgmma_i8" : "wgmma_f16");
+    case kPathTcgen05:
+      if (dtype == MM_DTYPE_BFLOAT16) return "wgmma_bf16";
+      return dtype == MM_DTYPE_FLOAT ? "wgmma_tf32" : (dtype == MM_DTYPE_UINT8 ? "wgmma_i8" : "wgmma_f16");
     case kPathDmma: return "dmma_f64";
     case kPathSemiring: return "semiring_simt";
   }

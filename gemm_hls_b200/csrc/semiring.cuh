@@ -8,6 +8,7 @@
 // reference's Naive<> (include/Utility.h:18-42) bit for bit.
 #pragma once
 
+#include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
 #include <cfloat>
@@ -67,6 +68,18 @@ struct Prim<__half> {
   static __device__ __forceinline__ __half min_value() { return __ushort_as_half(0x0400); }  // 2^-14
 };
 
+template <>
+struct Prim<__nv_bfloat16> {
+  static __device__ __forceinline__ __nv_bfloat16 add(__nv_bfloat16 a, __nv_bfloat16 b) { return __hadd_rn(a, b); }
+  static __device__ __forceinline__ __nv_bfloat16 mul(__nv_bfloat16 a, __nv_bfloat16 b) { return __hmul_rn(a, b); }
+  static __device__ __forceinline__ bool lt(__nv_bfloat16 a, __nv_bfloat16 b) { return __hlt(a, b); }
+  static __device__ __forceinline__ bool nz(__nv_bfloat16 a) { return __hneu(a, __ushort_as_bfloat16(0)); }  // true for NaN
+  static __device__ __forceinline__ __nv_bfloat16 zero() { return __ushort_as_bfloat16(0x0000); }
+  static __device__ __forceinline__ __nv_bfloat16 one() { return __ushort_as_bfloat16(0x3F80); }
+  static __device__ __forceinline__ __nv_bfloat16 max_value() { return __ushort_as_bfloat16(0x7F7F); }  // 0x1.fep127
+  static __device__ __forceinline__ __nv_bfloat16 min_value() { return __ushort_as_bfloat16(0x0080); }  // 2^-126
+};
+
 template <typename T>
 struct IntLimits;
 template <>
@@ -93,6 +106,7 @@ struct Lim {
 template <> struct Lim<float> : Prim<float> {};
 template <> struct Lim<double> : Prim<double> {};
 template <> struct Lim<__half> : Prim<__half> {};
+template <> struct Lim<__nv_bfloat16> : Prim<__nv_bfloat16> {};
 
 // ---- the functors (Operators.h) ---------------------------------------------------------------
 template <typename T>
@@ -170,6 +184,44 @@ struct PackedOpH<Product<__half>> {
   static __device__ __forceinline__ __half2 Apply2(__half2 a, __half2 b) { return __hmul2_rn(a, b); }
 };
 
+// bfloat16: the same with HADD2.BF16 / HMUL2.BF16 (__hadd2_rn / __hmul2_rn, never contracted into an HFMA2.BF16).
+template <class Op>
+struct PackedOpB {
+  static constexpr bool value = false;
+};
+template <>
+struct PackedOpB<Sum<__nv_bfloat16>> {
+  static constexpr bool value = true;
+  static __device__ __forceinline__ __nv_bfloat162 Apply2(__nv_bfloat162 a, __nv_bfloat162 b) { return __hadd2_rn(a, b); }
+};
+template <>
+struct PackedOpB<Product<__nv_bfloat16>> {
+  static constexpr bool value = true;
+  static __device__ __forceinline__ __nv_bfloat162 Apply2(__nv_bfloat162 a, __nv_bfloat162 b) { return __hmul2_rn(a, b); }
+};
+
+// The pair type of a 2-byte floating-point T and its conversions: broadcast, (low, high) -> pair, pair -> low / high.
+template <typename T>
+struct Packed2 {
+  using type = __half2;  // placeholder for the types without a packed path
+};
+template <>
+struct Packed2<__half> {
+  using type = __half2;
+  static __device__ __forceinline__ __half2 bcast(__half x) { return __half2half2(x); }
+  static __device__ __forceinline__ __half2 pair(__half lo, __half hi) { return __halves2half2(lo, hi); }
+  static __device__ __forceinline__ __half lo(__half2 x) { return __low2half(x); }
+  static __device__ __forceinline__ __half hi(__half2 x) { return __high2half(x); }
+};
+template <>
+struct Packed2<__nv_bfloat16> {
+  using type = __nv_bfloat162;
+  static __device__ __forceinline__ __nv_bfloat162 bcast(__nv_bfloat16 x) { return __bfloat162bfloat162(x); }
+  static __device__ __forceinline__ __nv_bfloat162 pair(__nv_bfloat16 lo, __nv_bfloat16 hi) { return __halves2bfloat162(lo, hi); }
+  static __device__ __forceinline__ __nv_bfloat16 lo(__nv_bfloat162 x) { return __low2bfloat16(x); }
+  static __device__ __forceinline__ __nv_bfloat16 hi(__nv_bfloat162 x) { return __high2bfloat16(x); }
+};
+
 // internal operator codes (never cross the C-ABI)
 enum { MM_OP_MIN_FAST = 5, MM_OP_MAX_FAST = 6 };
 
@@ -191,5 +243,6 @@ template <> struct DTypeOf<MM_DTYPE_DOUBLE> { using type = double; };
 template <> struct DTypeOf<MM_DTYPE_INT32> { using type = int; };
 template <> struct DTypeOf<MM_DTYPE_UINT32> { using type = unsigned; };
 template <> struct DTypeOf<MM_DTYPE_UINT8> { using type = unsigned char; };
+template <> struct DTypeOf<MM_DTYPE_BFLOAT16> { using type = __nv_bfloat16; };
 
 }  // namespace mm

@@ -50,6 +50,7 @@ int launch_semiring(int dtype, int map_op, int reduce_op, const GemmArgs &g_in) 
     case MM_DTYPE_INT32: rc = by_map<int>(map_op, reduce_op, g, ta, ring); break;
     case MM_DTYPE_UINT32: rc = by_map<unsigned>(map_op, reduce_op, g, ta, ring); break;
     case MM_DTYPE_UINT8: rc = by_map<unsigned char>(map_op, reduce_op, g, ta, ring); break;
+    case MM_DTYPE_BFLOAT16: rc = by_map<__nv_bfloat16>(map_op, reduce_op, g, ta, ring); break;
     default: return fail(MM_ERR_INVALID, "unknown data type");
   }
   if (rc < 0) return fail(MM_ERR_INVALID, "unknown map/reduce operator");

@@ -74,12 +74,19 @@ template <typename T, class Map, class Reduce>
 struct SemiringHalf2 {
   static constexpr bool value = std::is_same<T, __half>::value && PackedOpH<Map>::value && PackedOpH<Reduce>::value;
 };
+// bfloat16 likewise, as __nv_bfloat162 pairs (HADD2.BF16 / HMUL2.BF16).
+template <typename T, class Map, class Reduce>
+struct SemiringBf162 {
+  static constexpr bool value =
+      std::is_same<T, __nv_bfloat16>::value && PackedOpB<Map>::value && PackedOpB<Reduce>::value;
+};
 
-// 2 CTAs (16 warps) per SM for 4-byte element types and packed half: 64 accumulators + two k-steps of fragments fit
+// 2 CTAs (16 warps) per SM for 4-byte element types and packed half / bfloat16: 64 accumulators + two k-steps of fragments fit
 // in 128 registers without spilling.  8-byte types need the full 255-register budget, and unpacked 1- and
 // 2-byte types (one 32-bit register per element) spill at 128: those run 1 CTA per SM.
 template <typename T, class Map, class Reduce>
-__global__ void __launch_bounds__(256, (sizeof(T) == 4 || SemiringHalf2<T, Map, Reduce>::value) ? 2 : 1)
+__global__ void __launch_bounds__(256, (sizeof(T) == 4 || SemiringHalf2<T, Map, Reduce>::value ||
+                                       SemiringBf162<T, Map, Reduce>::value) ? 2 : 1)
 semiring_tile_kernel(const T *__restrict__ A, const __grid_constant__ CUtensorMap tmap_b, T *__restrict__ C,
                      unsigned size_n, unsigned size_k, unsigned size_m,
                      bool TRANSPOSED_A, unsigned a_step, unsigned b_step) {
@@ -101,16 +108,21 @@ semiring_tile_kernel(const T *__restrict__ A, const __grid_constant__ CUtensorMa
   const size_t row0 = size_t(blockIdx.y) * BM;
   const size_t col0 = size_t(blockIdx.x) * BN;
 
-  constexpr bool kHalf2 = SemiringHalf2<T, Map, Reduce>::value;
+  constexpr bool kBf162 = SemiringBf162<T, Map, Reduce>::value;
+  constexpr bool kHalf2 = SemiringHalf2<T, Map, Reduce>::value || kBf162;  // a packed pair path
+  using P2 = Packed2<T>;
+  using T2 = typename P2::type;
+  using MapOp2 = typename std::conditional<kBf162, PackedOpB<Map>, PackedOpH<Map>>::type;
+  using ReduceOp2 = typename std::conditional<kBf162, PackedOpB<Reduce>, PackedOpH<Reduce>>::type;
   T acc[8][8];
-  __half2 acc2[8][4];  // kHalf2 only: columns (2p, 2p + 1) of row i
+  T2 acc2[8][4];  // kHalf2 only: columns (2p, 2p + 1) of row i
 #pragma unroll
   for (int i = 0; i < 8; ++i) {
 #pragma unroll
     for (int j = 0; j < 8; ++j) acc[i][j] = Reduce::identity();
     if constexpr (kHalf2) {
 #pragma unroll
-      for (int p = 0; p < 4; ++p) acc2[i][p] = __half2half2(Reduce::identity());
+      for (int p = 0; p < 4; ++p) acc2[i][p] = P2::bcast(Reduce::identity());
     }
   }
 
@@ -214,20 +226,21 @@ semiring_tile_kernel(const T *__restrict__ A, const __grid_constant__ CUtensorMa
         }
       }
       if constexpr (kHalf2) {
-        // half, Map and Reduce in {Sum, Product}: two adjacent columns per HMUL2 / HADD2 (A element broadcast by
-        // the instruction's half selector), one rounding per Map and per Reduce per element, in Naive<>'s order
-        __half2 bp[2][4];
+        // half / bfloat16, Map and Reduce in {Sum, Product}: two adjacent columns per HMUL2 / HADD2 (A element
+        // broadcast by the instruction's half selector), one rounding per Map and per Reduce per element, in
+        // Naive<>'s order
+        T2 bp[2][4];
 #pragma unroll
         for (int u = 0; u < 2; ++u)
 #pragma unroll
-          for (int p = 0; p < 4; ++p) bp[u][p] = __halves2half2(bf[u][2 * p], bf[u][2 * p + 1]);
+          for (int p = 0; p < 4; ++p) bp[u][p] = P2::pair(bf[u][2 * p], bf[u][2 * p + 1]);
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
-          const __half2 a0 = __half2half2(af[0][i]), a1 = __half2half2(af[1][i]);
+          const T2 a0 = P2::bcast(af[0][i]), a1 = P2::bcast(af[1][i]);
 #pragma unroll
           for (int p = 0; p < 4; ++p) {
-            const __half2 t0 = PackedOpH<Map>::Apply2(a0, bp[0][p]), t1 = PackedOpH<Map>::Apply2(a1, bp[1][p]);
-            acc2[i][p] = PackedOpH<Reduce>::Apply2(PackedOpH<Reduce>::Apply2(acc2[i][p], t0), t1);
+            const T2 t0 = MapOp2::Apply2(a0, bp[0][p]), t1 = MapOp2::Apply2(a1, bp[1][p]);
+            acc2[i][p] = ReduceOp2::Apply2(ReduceOp2::Apply2(acc2[i][p], t0), t1);
           }
         }
       } else {
@@ -261,7 +274,7 @@ semiring_tile_kernel(const T *__restrict__ A, const __grid_constant__ CUtensorMa
 #pragma unroll
         for (int q = 0; q < 4; ++q) {
           if constexpr (kHalf2) {
-            out.v[q] = (q % 2 == 0) ? __low2half(acc2[i][h * 2 + q / 2]) : __high2half(acc2[i][h * 2 + q / 2]);
+            out.v[q] = (q % 2 == 0) ? P2::lo(acc2[i][h * 2 + q / 2]) : P2::hi(acc2[i][h * 2 + q / 2]);
           } else {
             out.v[q] = acc[i][h * 4 + q];
           }

@@ -39,7 +39,9 @@ enum {
   MM_DTYPE_INT32 = 3,  /* "int"    */
   MM_DTYPE_UINT32 = 4, /* "unsigned" */
   MM_DTYPE_UINT8 = 5,  /* "uint8_t" (reference CMakeLists.txt:43-46) */
-  MM_DTYPE_COUNT = 6
+  MM_DTYPE_BFLOAT16 = 6, /* bfloat16 (8-bit exponent, 8-bit significand): a library-level extension; the
+                          * reference has no such type.  Size 2, memory width 32, as half. */
+  MM_DTYPE_COUNT = 7
 };
 
 /* MM_MAP_OP / MM_REDUCE_OP = hlslib::op functors (hlslib/include/hlslib/xilinx/Operators.h:20-100).
@@ -77,6 +79,11 @@ enum {
    *     more than 1e-3 at K = 32 and 63 % at K = 544.  The reference's TestSimulation compares half
    *     EXACTLY (test/TestSimulation.cpp:79-85), so the host executables of this project build half
    *     with MM_FLAG_EXACT unless configured with -DMM_HALF_TENSOR=ON (INTEGRATION.md section 3).
+   *   - bfloat16 (Multiply, Add): bf16 wgmma with FP32 accumulation and ONE rounding to bfloat16 at the
+   *     end (round to nearest even).  Unlike a Naive<bfloat16>, it does not accumulate in bfloat16.  Under
+   *     MM_FLAG_EXACT, and for every other semiring, bfloat16 is BIT-IDENTICAL to a Naive<> that rounds to
+   *     bfloat16 after every Map and every Reduce.  Min / Max are the literal `(a < b) ? a : b`, as for half.
+   *     MM_FLAG_TF32X3 and the tf32_no_round knob do not apply.
    *   - uint8_t (Multiply, Add): u8 wgmma, exact 32-bit integer accumulation, low byte stored — BIT-IDENTICAL
    *     to the reference's modulo-256 arithmetic.  Used for K <= 33024 (255^2 * K < 2^31); the CUDA-core kernel beyond.
    *   - float Min / Max (as Map or Reduce): the hardware FMNMX.  Identical to the reference's
@@ -187,7 +194,7 @@ MM_API int mm_context_profile_read(mm_context *ctx, double *prep_seconds_sum,
 MM_API int mm_kernel_launch_count(int dtype, int map_op, int reduce_op, int flags);
 
 /* Name of the compute kernel family mm_kernel_enqueue() would dispatch to for a small problem
- * ("wgmma_tf32", "wgmma_f16", "wgmma_i8", "dmma_f64", "semiring_simt"); static string. */
+ * ("wgmma_tf32", "wgmma_f16", "wgmma_bf16", "wgmma_i8", "dmma_f64", "semiring_simt"); static string. */
 MM_API const char *mm_kernel_path(int dtype, int map_op, int reduce_op, int flags);
 
 /* The reference's simulation entry, extern "C" MatrixMultiplicationKernel(a, b, c, n, k, m)

@@ -10,6 +10,9 @@ import numpy as np  # noqa: E402
 import gemm_hls_b200 as G  # noqa: E402
 import oracle as O  # noqa: E402
 
+sys.path.insert(0, os.path.join(ROOT, "tests"))
+import bf16_naive  # noqa: E402  (bfloat16 has no reference Naive<>: the test suite's restatement)
+
 # (name, dtype, map, reduce, flags, (n, k, m)[, tuning])
 CASES = [
     ("wgmma_tf32", G.FLOAT, G.MULTIPLY, G.ADD, 0, (257, 48, 272)),
@@ -32,7 +35,25 @@ CASES = [
     ("semiring u8 exact", G.UINT8, G.MULTIPLY, G.ADD, G.FLAG_EXACT, (65, 128, 192)),
     ("semiring f16 exact", G.HALF, G.MULTIPLY, G.ADD, G.FLAG_EXACT, (65, 64, 96)),
     ("semiring f64 addmax TA", G.DOUBLE, G.ADD, G.MAX, G.FLAG_TRANSPOSED_A, (67, 16, 24)),
+    ("wgmma_bf16", G.BFLOAT16, G.MULTIPLY, G.ADD, 0, (257, 96, 288)),
+    ("wgmma_bf16 TA, 1 CTA, direct stores", G.BFLOAT16, G.MULTIPLY, G.ADD, G.FLAG_TRANSPOSED_A, (130, 64, 192),
+     dict(cta_group=1, tma_store=0)),
+    ("semiring bf16 exact", G.BFLOAT16, G.MULTIPLY, G.ADD, G.FLAG_EXACT, (65, 64, 96)),
+    ("semiring bf16 addmin", G.BFLOAT16, G.ADD, G.MIN, 0, (65, 64, 96)),
+    ("semiring bf16 addmax TA", G.BFLOAT16, G.ADD, G.MAX, G.FLAG_TRANSPOSED_A, (67, 32, 64)),
 ]
+
+
+def bf16_within_one_ulp(c, a, b, n, k, m, transposed):
+    """bf16 tensor path: every element within 1 ulp of an FP64 evaluation of the same inputs."""
+    def f(x):
+        return (np.asarray(x, dtype=np.uint16).astype(np.uint32) << 16).view(np.float32).astype(np.float64)
+    av = f(a).reshape((k, n) if transposed else (n, k))
+    ref = (av.T if transposed else av) @ f(b).reshape(k, m)
+    ulp = 2.0 ** (np.floor(np.log2(np.maximum(np.abs(ref), 2.0 ** -126))) - 7)
+    return bool(np.all(np.abs(f(c).reshape(n, m) - ref) <= ulp))
+
+
 only = os.environ.get("SANITIZE_ONLY")  # substring filter on the case name, e.g. SANITIZE_ONLY=dmma
 bad = 0
 for case in CASES:
@@ -40,14 +61,21 @@ for case in CASES:
     tuning = case[6] if len(case) > 6 else {}
     if only and only not in name:
         continue
-    a, b = O.fill(dt, n, k, m, 3)
+    a, b = bf16_naive.fill(O, n, k, m, 3) if dt == G.BFLOAT16 else O.fill(dt, n, k, m, 3)
     if dt == G.HALF:
         a = (a.astype(np.float32) * np.float32(0.25)).astype(np.float16)
     with G.Context(0) as ctx:
         ctx.set_tuning(**tuning)
         c = ctx.gemm_host(dt, mp, rd, a, b, n, k, m, flags=flags)[0]
-    ref = O.naive(dt, mp, rd, a, b, n, k, m, transposed_a=bool(flags & G.FLAG_TRANSPOSED_A), threads=4)
-    ok = O.verify(dt, c, ref) == -1 if G.kernel_path(dt, mp, rd, flags) == "semiring_simt" or dt != G.HALF else True
+    if dt == G.BFLOAT16:
+        ta = bool(flags & G.FLAG_TRANSPOSED_A)
+        if G.kernel_path(dt, mp, rd, flags) == "semiring_simt":
+            ok = bf16_naive.same_nan_free(c, bf16_naive.naive(mp, rd, a, b, n, k, m, transposed_a=ta))
+        else:
+            ok = bf16_within_one_ulp(c, a, b, n, k, m, ta)
+    else:
+        ref = O.naive(dt, mp, rd, a, b, n, k, m, transposed_a=bool(flags & G.FLAG_TRANSPOSED_A), threads=4)
+        ok = O.verify(dt, c, ref) == -1 if G.kernel_path(dt, mp, rd, flags) == "semiring_simt" or dt != G.HALF else True
     print("%-42s %s" % (name, "ok" if ok else "MISMATCH"), flush=True)
     bad += 0 if ok else 1
 # batched calls (3 ragged problems, packed or shared operands): every problem equals its single call
@@ -64,6 +92,10 @@ BATCHED = [
     ("batched semiring f32 addmin shared B", G.FLOAT, G.ADD, G.MIN, G.FLAG_BATCH_SHARED_B, (129, 48, 144)),
     ("batched semiring i32 staged kernel", G.INT32, G.MULTIPLY, G.ADD, 0, (65, 32, 48), dict(semiring_ring=0)),
     ("batched semiring f64 addmax TA", G.DOUBLE, G.ADD, G.MAX, G.FLAG_TRANSPOSED_A, (67, 16, 24)),
+    ("batched wgmma_bf16 shared A", G.BFLOAT16, G.MULTIPLY, G.ADD, G.FLAG_BATCH_SHARED_A, (129, 96, 288)),
+    ("batched wgmma_bf16 TA, shared B", G.BFLOAT16, G.MULTIPLY, G.ADD, G.FLAG_TRANSPOSED_A | G.FLAG_BATCH_SHARED_B,
+     (130, 64, 192)),
+    ("batched semiring bf16 addmin", G.BFLOAT16, G.ADD, G.MIN, 0, (65, 64, 96)),
 ]
 shared_flags = G.FLAG_BATCH_SHARED_A | G.FLAG_BATCH_SHARED_B
 for case in BATCHED:
@@ -74,7 +106,7 @@ for case in BATCHED:
     batch = 3
     na = 1 if flags & G.FLAG_BATCH_SHARED_A else batch
     nb = 1 if flags & G.FLAG_BATCH_SHARED_B else batch
-    data = [O.fill(dt, n, k, m, 40 + i) for i in range(batch)]
+    data = [bf16_naive.fill(O, n, k, m, 40 + i) if dt == G.BFLOAT16 else O.fill(dt, n, k, m, 40 + i) for i in range(batch)]
     a = np.concatenate([d[0].reshape(-1) for d in data[:na]])
     b = np.concatenate([d[1].reshape(-1) for d in data[:nb]])
     if dt == G.HALF:
@@ -99,9 +131,10 @@ for case in BATCHED:
     bad += 0 if ok else 1
 # the row-block split on one device listed twice: sliced upload of B, the gather kernel, host barriers
 if not only or "multi" in only:
-    for dt, shape in ((G.FLOAT, (300, 128, 272)), (G.HALF, (257, 128, 288)), (G.DOUBLE, (130, 128, 136))):
+    for dt, shape in ((G.FLOAT, (300, 128, 272)), (G.HALF, (257, 128, 288)), (G.DOUBLE, (130, 128, 136)),
+                      (G.BFLOAT16, (257, 128, 288))):
         n, k, m = shape
-        a, b = O.fill(dt, n, k, m, 5)
+        a, b = bf16_naive.fill(O, n, k, m, 5) if dt == G.BFLOAT16 else O.fill(dt, n, k, m, 5)
         if dt == G.HALF:
             a = (a.astype(np.float32) * np.float32(0.25)).astype(np.float16)
         single = G.matrix_multiplication_kernel(a, b, n, k, m, dtype=dt)
