@@ -48,10 +48,14 @@
 namespace mm {
 namespace {
 
+// Round to nearest TF32, ties away from zero.  cvt.rna rounds every finite |x| >= 0x7F7FF000 up to
+// infinity; a finite operand must stay finite (x * 0.5 is finite), so those saturate to the largest
+// finite TF32 value, +-0x7F7FE000.  Infinities and NaN pass through.
 __device__ __forceinline__ float round_tf32(float x) {
   uint32_t r;
   asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
-  return __uint_as_float(r);
+  const bool overflowed = (r & 0x7FFFFFFFu) == 0x7F800000u && (__float_as_uint(x) & 0x7FFFFFFFu) != 0x7F800000u;
+  return __uint_as_float(overflowed ? ((r & 0x80000000u) | 0x7F7FE000u) : r);
 }
 
 // ---- operand preparation ------------------------------------------------------------------------
@@ -184,12 +188,18 @@ transpose_prep_kernel(const T *__restrict__ src, T *__restrict__ dst, uint32_t s
 // (the dropped lo*lo term is 2^-22 relative).  The three products are folded into ONE GEMM with
 // K' = 3K by interleaving 16-element k-blocks:  A' = [hi | hi | lo],  B'^T = [hi | lo | hi],
 // so the unchanged wgmma kernel accumulates all three in its FP32 register accumulators.
+// Infinities: lo = 0 (inf - inf would be NaN), and the hi that meets the other operand's lo (A's second
+// block, B's third) carries 0 in place of +-inf (inf * 0 would be NaN where the other operand is exactly
+// TF32).  Only hi * hi carries infinities, so C gets IEEE's +-inf; NaN still propagates through hi.
 constexpr int SPLIT_BLOCK = 16;  // K % 16 == 0 by the reference's shape rule for float
 
 __device__ __forceinline__ void split_tf32(float x, float &hi, float &lo) {
   hi = round_tf32(x);
-  lo = round_tf32(x - hi);
+  lo = isinf(x) ? 0.0f : round_tf32(x - hi);
 }
+
+// hi for the cross terms: +-inf -> 0
+__device__ __forceinline__ float finite_or_zero(float hi) { return isinf(hi) ? 0.0f : hi; }
 
 // dst[r][3K]: per 16-block of k -> [hi16 | hi16 | lo16]; one thread per float4 of the source row.
 __global__ void __launch_bounds__(256)
@@ -209,13 +219,15 @@ split3_rows_kernel(const float4 *__restrict__ src, float4 *__restrict__ dst, siz
     split_tf32(v.w, hi.w, lo.w);
     float4 *row = dst + r * (3 * k4) + size_t(blk) * (3 * SPLIT_BLOCK / 4) + in;
     row[0] = hi;
-    row[SPLIT_BLOCK / 4] = hi;
+    row[SPLIT_BLOCK / 4] = make_float4(finite_or_zero(hi.x), finite_or_zero(hi.y), finite_or_zero(hi.z),
+                                       finite_or_zero(hi.w));
     row[2 * SPLIT_BLOCK / 4] = lo;
   }
 }
 
 // src (src_rows = K) x (src_cols) row-major -> dst[c][3K] with per-16-block [a | b | c] where
-// B_ORDER selects (hi, lo, hi) for the B operand and (hi, hi, lo) for a transposed A.  blockIdx.z =
+// B_ORDER selects (hi, lo, hi') for the B operand and (hi, hi', lo) for a transposed A, hi' =
+// finite_or_zero(hi).  blockIdx.z =
 // problem of a batch, as in transpose_prep_kernel.
 template <bool B_ORDER>
 __global__ void __launch_bounds__(256)
@@ -244,8 +256,8 @@ split3_transpose_kernel(const float *__restrict__ src, float *__restrict__ dst, 
       float *out = dst + size_t(c) * (3 * size_t(src_rows)) + size_t(r / SPLIT_BLOCK) * (3 * SPLIT_BLOCK) +
                    (r % SPLIT_BLOCK);
       out[0] = hi;
-      out[SPLIT_BLOCK] = B_ORDER ? lo : hi;
-      out[2 * SPLIT_BLOCK] = B_ORDER ? hi : lo;
+      out[SPLIT_BLOCK] = B_ORDER ? lo : finite_or_zero(hi);
+      out[2 * SPLIT_BLOCK] = B_ORDER ? finite_or_zero(hi) : lo;
     }
   }
 }
