@@ -289,10 +289,14 @@ class Multi:
         _check(lib().mm_multi_execute(self._h, dtype, map_op, reduce_op, flags, n, k, m, ctypes.byref(sd), ctypes.byref(sw)))
         return sd.value, sw.value
 
-    def download(self, dtype, n, m):
-        c = np.empty((n, m), dtype=NP_DTYPE[dtype])
-        _check(lib().mm_multi_download(self._h, dtype, c.ctypes.data, n, m))
-        return c
+    def download(self, dtype, n, m, out=None):
+        """C of the last execute into `out` (a C-contiguous array of n*m elements of the type), or a new array."""
+        if out is None:
+            out = np.empty((n, m), dtype=NP_DTYPE[dtype])
+        elif not out.flags["C_CONTIGUOUS"] or out.nbytes != n * m * int(lib().mm_dtype_size(dtype)):
+            raise MMError(1, "out must be a C-contiguous array of n*m elements of the type")
+        _check(lib().mm_multi_download(self._h, dtype, out.ctypes.data, n, m))
+        return out
 
 
 def _host_operand(dtype, x):
@@ -323,9 +327,10 @@ def _gemm_host(handle, dtype, map_op, reduce_op, a, b, n, k, m, flags, out, fn=N
     return c, sd.value, sw.value
 
 
-def matrix_multiplication_kernel(a, b, n, k, m, dtype=FLOAT, map_op=MULTIPLY, reduce_op=ADD, flags=0):
+def matrix_multiplication_kernel(a, b, n, k, m, dtype=FLOAT, map_op=MULTIPLY, reduce_op=ADD, flags=0, out=None):
     """The reference's ``MatrixMultiplicationKernel(a, b, c, n, k, m)`` called with host pointers
     (test/TestSimulation.cpp:66), for a run-time chosen (MM_DATA_TYPE, MM_MAP_OP, MM_REDUCE_OP).
-    Returns C as an (n, m) numpy array.  Uses the library's default context on device 0."""
-    c, _, _ = _gemm_host(None, dtype, map_op, reduce_op, a, b, n, k, m, flags, None)
+    Returns C as an (n, m) numpy array (`out`, the reference's c, when given).  Uses the library's
+    default context on device 0."""
+    c, _, _ = _gemm_host(None, dtype, map_op, reduce_op, a, b, n, k, m, flags, out)
     return c

@@ -95,6 +95,7 @@ struct mm_context {
   cudaEvent_t ev_slice = nullptr;                      // multi-GPU: this device's slice of B has arrived
   mm::Scratch scratch;       // operand copies of the tensor-core path
   mm::Scratch staging[3];    // device A, B, C of the host-pointer entries
+  uint64_t staging_gen = 0;  // bumped by every call that writes staging[]: mm_multi_* checks its upload is still there
   std::vector<void *> retired;  // superseded scratch allocations a captured graph may still reference
   bool captured = false;        // a stream capture has gone through this context
   mm::Tuning tuning;
@@ -323,6 +324,7 @@ struct Pipeline {
   // Phase 1: allocations + this device's (slice of) B on its way.  Records ctx->ev_slice.
   int upload_b(const BPlan &bp) {
     MM_CUDA_TRY(cudaSetDevice(ctx->device));
+    ++ctx->staging_gen;
     int rc;
     if ((rc = ensure(ctx, ctx->staging[0], size_t(rows) * k * es, false)) != MM_OK) return rc;
     if ((rc = ensure(ctx, ctx->staging[1], size_t(k) * m * es, false)) != MM_OK) return rc;
@@ -497,9 +499,12 @@ struct mm_multi {
   std::vector<void **> parts_dev;  // per device: device array of G pointers to the devices' B buffers
   bool peer = false;
   std::mutex mutex;
-  // resident problem of the upload / execute / download lifecycle
+  // resident problem of the upload / execute / download lifecycle: valid while every device's staging
+  // generation is the one its upload left (no other call has written those buffers since)
   unsigned n = 0, k = 0, m = 0;
   int dtype = -1;
+  std::vector<uint64_t> gen;
+  bool executed = false;  // an execute has run on the resident operands since the upload
 };
 
 namespace {
@@ -614,6 +619,28 @@ int multi_gemm_host_locked(mm_multi *mu, int dtype, int map_op, int reduce_op, i
   return MM_OK;
 }
 
+void clear_resident(mm_multi *mu) {
+  mu->n = mu->k = mu->m = 0;
+  mu->dtype = -1;
+  mu->gen.clear();
+  mu->executed = false;
+}
+
+// The resident problem of mm_multi_upload is (dtype, n, k, m) and still sits in every device's staging buffers.
+int check_resident(mm_multi *mu, const char *entry, int dtype, unsigned n, unsigned k, unsigned m) {
+  if (mu->dtype != dtype || mu->n != n || mu->k != k || mu->m != m) {
+    return fail(MM_ERR_INVALID, std::string(entry) + ": no matching mm_multi_upload (type or sizes differ)");
+  }
+  for (size_t g = 0; g < mu->ctx.size(); ++g) {
+    std::lock_guard<std::mutex> lock(mu->ctx[g]->mutex);
+    if (mu->ctx[g]->staging_gen != mu->gen[g]) {
+      return fail(MM_ERR_INVALID, std::string(entry) + ": no matching mm_multi_upload (GPU " + std::to_string(g) +
+                                      "'s buffers were reused by another call since)");
+    }
+  }
+  return MM_OK;
+}
+
 int create_multi(int n_gpus, const int *devices, mm_multi **out) {
   mm_multi *mu = new mm_multi();
   auto cleanup = [&](int rc) {
@@ -660,7 +687,7 @@ extern "C" {
 
 const char *mm_last_error(void) { return mm::g_last_error.c_str(); }
 
-int mm_version(void) { return 202; }
+int mm_version(void) { return 203; }
 
 size_t mm_dtype_size(int dtype) {
   switch (dtype) {
@@ -1019,18 +1046,21 @@ int mm_multi_gemm_host(mm_multi *mu, int dtype, int map_op, int reduce_op, int f
 int mm_multi_upload(mm_multi *mu, int dtype, int flags, const void *a, const void *b, unsigned n, unsigned k,
                     unsigned m) {
   if (!mu) return fail(MM_ERR_INVALID, "null multi-GPU context");
+  std::lock_guard<std::mutex> lock(mu->mutex);
+  clear_resident(mu);  // a failed upload, rejected arguments included, leaves no resident problem behind
   int rc = check_args(dtype, MM_OP_MULTIPLY, MM_OP_ADD, a, b, a /*non-null placeholder*/, n, k, m);
   if (rc != MM_OK) return rc;
   if (flags & MM_FLAG_TRANSPOSED_A) {
     return fail(MM_ERR_UNSUPPORTED, "the row-block split over GPUs needs row-major A (MM_TRANSPOSED_A is set)");
   }
-  std::lock_guard<std::mutex> lock(mu->mutex);
   const int G = int(mu->ctx.size());
   const size_t es = mm_dtype_size(dtype);
+  std::vector<uint64_t> gen(G, 0);
   HostBarrier barrier(G);
   rc = fan_out(G, [&](int g) -> int {
     mm_context *ctx = mu->ctx[g];
     std::lock_guard<std::mutex> ctx_lock(ctx->mutex);
+    gen[g] = ++ctx->staging_gen;
     const Partition part = partition_for(G, g, n, k, mu->peer);
     const unsigned r0 = part.r0, r1 = part.r1, part_rows = part.part_rows, parts = part.parts;
     const unsigned rows = std::max(1u, r1 - r0);
@@ -1086,6 +1116,7 @@ int mm_multi_upload(mm_multi *mu, int dtype, int flags, const void *a, const voi
   mu->k = k;
   mu->m = m;
   mu->dtype = dtype;
+  mu->gen = gen;
   return MM_OK;
 }
 
@@ -1094,13 +1125,13 @@ int mm_multi_execute(mm_multi *mu, int dtype, int map_op, int reduce_op, int fla
   if (!mu) return fail(MM_ERR_INVALID, "null multi-GPU context");
   if (!valid_dtype(dtype) || !valid_op(map_op) || !valid_op(reduce_op)) return fail(MM_ERR_INVALID, "unknown type / operator code");
   std::lock_guard<std::mutex> lock(mu->mutex);
-  if (mu->dtype != dtype || mu->n != n || mu->k != k || mu->m != m) {
-    return fail(MM_ERR_INVALID, "mm_multi_execute: no matching mm_multi_upload (type or sizes differ)");
-  }
+  int rc = check_resident(mu, "mm_multi_execute", dtype, n, k, m);
+  if (rc != MM_OK) return rc;
+  mu->executed = false;  // C is rewritten below: a failed execute leaves nothing to download
   const int G = int(mu->ctx.size());
   std::vector<double> dev_s(G, 0.0);
   const auto t0 = std::chrono::high_resolution_clock::now();
-  int rc = fan_out(G, [&](int g) -> int {
+  rc = fan_out(G, [&](int g) -> int {
     const Partition part = partition_for(G, g, n, k, mu->peer);
     const unsigned r0 = part.r0, r1 = part.r1;
     if (r1 == r0) return MM_OK;
@@ -1109,6 +1140,7 @@ int mm_multi_execute(mm_multi *mu, int dtype, int map_op, int reduce_op, int fla
                              ctx->staging[2].ptr, r1 - r0, k, m, &dev_s[g], nullptr);
   });
   if (rc != MM_OK) return rc;
+  mu->executed = true;
   if (seconds_device) *seconds_device = *std::max_element(dev_s.begin(), dev_s.end());
   if (seconds_wall) {
     *seconds_wall = std::chrono::duration<double>(std::chrono::high_resolution_clock::now() - t0).count();
@@ -1119,9 +1151,9 @@ int mm_multi_execute(mm_multi *mu, int dtype, int map_op, int reduce_op, int fla
 int mm_multi_download(mm_multi *mu, int dtype, void *c, unsigned n, unsigned m) {
   if (!mu || !c) return fail(MM_ERR_INVALID, "null argument");
   std::lock_guard<std::mutex> lock(mu->mutex);
-  if (mu->dtype != dtype || mu->n != n || mu->m != m) {
-    return fail(MM_ERR_INVALID, "mm_multi_download: no matching mm_multi_upload (type or sizes differ)");
-  }
+  const int rc = check_resident(mu, "mm_multi_download", dtype, n, mu->k, m);
+  if (rc != MM_OK) return rc;
+  if (!mu->executed) return fail(MM_ERR_INVALID, "mm_multi_download: no mm_multi_execute since the last upload");
   const int G = int(mu->ctx.size());
   const size_t es = mm_dtype_size(dtype);
   return fan_out(G, [&](int g) -> int {

@@ -292,7 +292,12 @@ MM_API int mm_multi_gemm_host(mm_multi *multi, int dtype, int map_op, int reduce
 /* Device-resident lifecycle, the multi-GPU form of MakeBuffer + CopyFromHost / ExecuteTask / CopyToHost
  * (host/RunHardware.cpp:122-190): upload = A row-blocks + B slices over PCIe, B assembled on every
  * GPU over NVLink; execute = the kernels of every GPU on the resident buffers (device seconds = the
- * slowest GPU's CUDA-event time around its kernels); download = C row-blocks to the host. */
+ * slowest GPU's CUDA-event time around its kernels); download = C row-blocks to the host.
+ * The resident operands live in the same per-device staging buffers that mm_multi_gemm_host() and mm_gemm_host()
+ * on a member context (mm_multi_context()) use.  Execute and download therefore return MM_ERR_INVALID, never
+ * MM_OK over other operands, unless the last upload on this multi succeeded, had the same type and sizes, and no
+ * call has reused any member context's staging buffers since.  Download also needs an execute after that upload.
+ * (Since version 203; earlier versions computed on, or returned, whatever those buffers held.) */
 MM_API int mm_multi_upload(mm_multi *multi, int dtype, int flags, const void *a_host, const void *b_host,
                            unsigned size_n, unsigned size_k, unsigned size_m);
 MM_API int mm_multi_execute(mm_multi *multi, int dtype, int map_op, int reduce_op, int flags,

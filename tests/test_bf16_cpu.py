@@ -24,10 +24,10 @@ MM_ERR_INVALID = 1
 
 # ---- static queries -----------------------------------------------------------------------------
 
-def test_static_queries(mm):
+def test_static_queries_of_version_203(mm):
     L = mm.lib()
     assert mm.BFLOAT16 == BF16
-    assert L.mm_version() == 202
+    assert L.mm_version() == 203
     assert L.mm_dtype_size(BF16) == 2 and mm.memory_width(BF16) == 32
     assert mm.kernel_path(BF16) == "wgmma_bf16"
     assert mm.launch_count(BF16) == 2                                   # B's K-major copy + GEMM, as half
