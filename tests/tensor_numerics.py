@@ -234,6 +234,30 @@ def exact_limit(path, k):
     return min(TYPE_INT_LIMIT[path], int(math.isqrt(EXACT_S_LIMIT // k)))
 
 
+# Exact data at the benchmark sizes (tests/test_full_size_exact_gpu.py): nonzero integers in [-limit, limit] times
+# 2^ea per row of A and 2^eb per column of B, ea and eb cycling through these inclusive ranges.  Every C element is
+# then an integer of magnitude <= limit^2 K times the one power of two 2^(ea + eb) of its row and column.  half:
+# |C| <= 2^22 2^(-4 - 3) < 2^15, and every nonzero |C| >= 2^(-6 - 6) = 2^-12, a normal half.
+_FULL_SIZE_EXP = {"tf32": ((-3, -1), (-2, 0)), "tf32x3": ((-3, -1), (-2, 0)), "f16": ((-6, -4), (-6, -3)),
+                  "bf16": ((-3, -1), (-2, 0)), "dmma": ((-3, -1), (-2, 0))}
+# Bound on limit^2 K: the FP32-accumulating paths keep 2 bits of FP32's 24 to spare (EXACT_S_LIMIT); DMMA
+# accumulates in FP64 and keeps the same 2 bits of FP64's 53, so it takes the type's whole exact range (1024).
+FULL_SIZE_S_LIMIT = {"tf32": EXACT_S_LIMIT, "tf32x3": EXACT_S_LIMIT, "f16": EXACT_S_LIMIT, "bf16": EXACT_S_LIMIT,
+                     "dmma": 2 ** 51}
+
+
+def full_size_scheme(path, k):
+    """(limit, (ea_lo, ea_hi), (eb_lo, eb_hi)) of the exact data of `path` at inner extent k: the largest integer
+    magnitude with limit^2 k <= FULL_SIZE_S_LIMIT[path] within the type's exact range, and the exponent ranges of
+    the row scales of A and the column scales of B.  uint8: (255, None, None), full-range bytes, whose products and
+    sums are exact in the 32-bit accumulator (255^2 k < 2^31)."""
+    if path == "u8":
+        return 255, None, None
+    lim = min(TYPE_INT_LIMIT[path], int(math.isqrt(FULL_SIZE_S_LIMIT[path] // k)))
+    ea, eb = _FULL_SIZE_EXP[path]
+    return lim, ea, eb
+
+
 def _nonzero_ints(rng, lim, shape):
     return rng.integers(1, lim + 1, size=shape) * rng.choice(np.array([-1, 1]), size=shape)
 
