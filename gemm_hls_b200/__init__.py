@@ -26,6 +26,7 @@ MULTIPLY, ADD, MIN, MAX, AND = range(5)
 # flags
 FLAG_NONE, FLAG_TRANSPOSED_A, FLAG_EXACT, FLAG_TF32X3 = 0, 1, 2, 4
 FLAG_BATCH_SHARED_A, FLAG_BATCH_SHARED_B = 8, 16   # batched calls: every problem reads the same A / B
+WITNESS_NONE = 0xFFFFFFFF   # MM_WITNESS_NONE: the reduction never selected a term (Context.enqueue_witness)
 
 # numpy has no bfloat16: BFLOAT16 host arrays are its bit patterns (np.uint16, or ml_dtypes.bfloat16), taken by view
 NP_DTYPE = {HALF: np.float16, FLOAT: np.float32, DOUBLE: np.float64,
@@ -49,7 +50,7 @@ EXPORTS = ["mm_last_error", "mm_version", "mm_dtype_size", "mm_memory_width", "m
            "mm_copy_to_host", "mm_kernel_execute", "mm_kernel_enqueue", "mm_kernel_launch_count",
            "mm_kernel_path", "mm_gemm_host", "mm_context_set_profiling", "mm_context_profile_read",
            "mm_context_set_tuning", "mm_context_get_tuning", "mm_context_reserve",
-           "mm_kernel_enqueue_batched", "mm_context_reserve_batched",
+           "mm_kernel_enqueue_batched", "mm_context_reserve_batched", "mm_kernel_enqueue_witness",
            "mm_multi_create", "mm_multi_destroy", "mm_multi_device_count", "mm_multi_context",
            "mm_multi_peer_access", "mm_multi_partition", "mm_multi_gemm_host", "mm_multi_upload", "mm_multi_execute",
            "mm_multi_download"]
@@ -97,6 +98,7 @@ def lib():
         L.mm_context_reserve.argtypes = [vp, i, i, u, u, u]
         L.mm_kernel_enqueue_batched.argtypes = [vp, i, i, i, i, vp, vp, vp, u, u, u, u, vp]
         L.mm_context_reserve_batched.argtypes = [vp, i, i, u, u, u, u]
+        L.mm_kernel_enqueue_witness.argtypes = [vp, i, i, i, i, vp, vp, vp, vp, u, u, u, u, vp]
         L.mm_multi_create.argtypes = [i, ctypes.POINTER(i), ctypes.POINTER(vp)]
         L.mm_multi_destroy.argtypes = [vp]
         L.mm_multi_device_count.argtypes = [vp]
@@ -188,6 +190,13 @@ class Context:
         """`batch` packed problems (A at a + i*n*k, B at b + i*k*m unless FLAG_BATCH_SHARED_A / _B, C at
         c + i*n*m elements) in one asynchronous launch sequence; each C equals its single enqueue bit for bit."""
         _check(lib().mm_kernel_enqueue_batched(self._h, dtype, map_op, reduce_op, flags, a_dev, b_dev, c_dev,
+                                               n, k, m, batch, ctypes.c_void_p(stream) if stream else None))
+
+    def enqueue_witness(self, dtype, map_op, reduce_op, a_dev, b_dev, c_dev, w_dev, n, k, m, batch=1, flags=0,
+                        stream=None):
+        """C exactly as enqueue_batched computes it, plus W (n*m uint32 per problem, packed like C): for a Min or
+        Max reduce, the k whose term each element of C was selected from last, or WITNESS_NONE (include/mm_b200.h)."""
+        _check(lib().mm_kernel_enqueue_witness(self._h, dtype, map_op, reduce_op, flags, a_dev, b_dev, c_dev, w_dev,
                                                n, k, m, batch, ctypes.c_void_p(stream) if stream else None))
 
     def set_tuning(self, **knobs):

@@ -216,28 +216,42 @@ int check_batch(unsigned batch, unsigned n, unsigned k, unsigned m) {
   return MM_OK;
 }
 
+// Stream-capture and profiling bookkeeping of one enqueued call.  *pe = the call's three profiling events (start,
+// after preparation, after the main kernel; the start one already recorded), or null when `profile` is false or
+// profiling is off or full.
+int begin_call(mm_context *ctx, cudaStream_t stream, bool profile, cudaStreamCaptureStatus *capture,
+               cudaEvent_t **pe) {
+  *capture = cudaStreamCaptureStatusNone;
+  if (cudaStreamIsCapturing(stream, capture) == cudaSuccess && *capture != cudaStreamCaptureStatusNone) {
+    ctx->captured = true;
+  }
+  *pe = nullptr;
+  if (profile && ctx->profiling && ctx->prof_calls < 256) {
+    while (ctx->prof_events.size() < size_t(3 * (ctx->prof_calls + 1))) {
+      cudaEvent_t e;
+      MM_CUDA_TRY(cudaEventCreate(&e));
+      ctx->prof_events.push_back(e);
+    }
+    *pe = &ctx->prof_events[3 * ctx->prof_calls];
+    ++ctx->prof_calls;
+    MM_CUDA_TRY(cudaEventRecord((*pe)[0], stream));
+  }
+  return MM_OK;
+}
+
 int enqueue_locked(mm_context *ctx, int dtype, int map_op, int reduce_op, int flags, const void *a,
                    const void *b, void *c, unsigned n, unsigned k, unsigned m, cudaStream_t stream,
                    bool dry_run = false, unsigned batch = 1) {
   mm::GemmArgs g = make_args(ctx, a, b, c, n, k, m, flags, stream);
   g.batch = make_batch(batch, flags);
   g.dry_run = dry_run;
-  cudaStreamCaptureStatus capture = cudaStreamCaptureStatusNone;
-  if (cudaStreamIsCapturing(stream, &capture) == cudaSuccess && capture != cudaStreamCaptureStatusNone) {
-    ctx->captured = true;
-  }
-  cudaEvent_t *pe = nullptr;
-  if (!dry_run && ctx->profiling && ctx->prof_calls < 256) {
-    while (ctx->prof_events.size() < size_t(3 * (ctx->prof_calls + 1))) {
-      cudaEvent_t e;
-      MM_CUDA_TRY(cudaEventCreate(&e));
-      ctx->prof_events.push_back(e);
-    }
-    pe = &ctx->prof_events[3 * ctx->prof_calls];
-    ++ctx->prof_calls;
+  cudaStreamCaptureStatus capture;
+  cudaEvent_t *pe;
+  const int rc_begin = begin_call(ctx, stream, !dry_run, &capture, &pe);
+  if (rc_begin != MM_OK) return rc_begin;
+  if (pe) {
     g.ev_start = pe[0];
     g.ev_prep_done = pe[1];
-    MM_CUDA_TRY(cudaEventRecord(pe[0], stream));
   }
   int rc_launch = MM_OK;
   switch (select_path(dtype, map_op, reduce_op, flags, n, k)) {
@@ -848,6 +862,33 @@ int mm_kernel_enqueue_batched(mm_context *ctx, int dtype, int map_op, int reduce
   MM_CUDA_TRY(cudaSetDevice(ctx->device));
   cudaStream_t s = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ctx->stream;
   return enqueue_locked(ctx, dtype, map_op, reduce_op, flags, a, b, c, n, k, m, s, /*dry_run=*/false, batch);
+}
+
+int mm_kernel_enqueue_witness(mm_context *ctx, int dtype, int map_op, int reduce_op, int flags, const void *a,
+                              const void *b, void *c, unsigned *w, unsigned n, unsigned k, unsigned m, unsigned batch,
+                              void *cuda_stream) {
+  if (!ctx) return fail(MM_ERR_INVALID, "null context");
+  int rc = check_args(dtype, map_op, reduce_op, a, b, c, n, k, m);
+  if (rc != MM_OK) return rc;
+  if ((rc = check_batch(batch, n, k, m)) != MM_OK) return rc;
+  if ((rc = check_device_alignment(a, b, c)) != MM_OK) return rc;
+  if (!w) return fail(MM_ERR_INVALID, "null witness pointer");
+  if (reinterpret_cast<uintptr_t>(w) % 16 != 0) return fail(MM_ERR_INVALID, "the witness pointer must be 16-byte aligned");
+  if (reduce_op != MM_OP_MIN && reduce_op != MM_OP_MAX) {
+    return fail(MM_ERR_INVALID, "witnesses exist for the Min and Max reduces only");
+  }
+  std::lock_guard<std::mutex> lock(ctx->mutex);
+  MM_CUDA_TRY(cudaSetDevice(ctx->device));
+  cudaStream_t s = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ctx->stream;
+  mm::GemmArgs g = make_args(ctx, a, b, c, n, k, m, flags, s);
+  g.batch = make_batch(batch, flags);
+  cudaStreamCaptureStatus capture;
+  cudaEvent_t *pe;
+  if ((rc = begin_call(ctx, s, /*profile=*/true, &capture, &pe)) != MM_OK) return rc;
+  if (pe) MM_CUDA_TRY(cudaEventRecord(pe[1], s));  // like a semiring call: no preparation
+  if ((rc = mm::launch_semiring_witness(dtype, map_op, reduce_op, g, w)) != MM_OK) return rc;
+  if (pe) MM_CUDA_TRY(cudaEventRecord(pe[2], s));
+  return MM_OK;
 }
 
 int mm_kernel_execute(mm_context *ctx, int dtype, int map_op, int reduce_op, int flags,

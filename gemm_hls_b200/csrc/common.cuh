@@ -90,6 +90,8 @@ struct GemmArgs {
 // ---- kernel families (one launcher per translation unit) ---------------------------------------
 // CUDA-core semiring tile kernel, any (dtype, map, reduce).  semiring_*.cu
 int launch_semiring(int dtype, int map_op, int reduce_op, const GemmArgs &args);
+// The same C for a Min / Max reduce, plus the witness W (N x M uint32 per problem).  semiring_witness_*.cu
+int launch_semiring_witness(int dtype, int map_op, int reduce_op, const GemmArgs &args, unsigned *w);
 
 // wgmma tensor-core GEMM for (Multiply, Add) float (tf32), half (f16) and uint8_t (u8).
 // The context's scratch holds, in this order: [B operand copy][A operand copy][counters].

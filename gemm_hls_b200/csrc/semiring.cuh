@@ -164,6 +164,33 @@ struct MaxFast<float> {
   static __device__ __forceinline__ float identity() { return Lim<float>::min_value(); }
 };
 
+// ---- witnesses (mm_kernel_enqueue_witness) -------------------------------------------------------------
+// Selects<Reduce>::apply(acc, t): whether the step acc <- Reduce(acc, t) keeps the new term t.  The literal
+// `(acc < t) ? acc : t` keeps t unless acc is strictly better, so ties go to the later k and a NaN term is kept;
+// FMNMX keeps t only when it is strictly better, so ties go to the earlier k and a NaN term is dropped.
+template <class Reduce>
+struct Selects;
+template <typename T>
+struct Selects<Min<T>> {
+  static __device__ __forceinline__ bool apply(T acc, T t) { return !Prim<T>::lt(acc, t); }
+};
+template <typename T>
+struct Selects<Max<T>> {
+  static __device__ __forceinline__ bool apply(T acc, T t) { return !Prim<T>::lt(t, acc); }
+};
+template <typename T>
+struct Selects<MinFast<T>> : Selects<Min<T>> {};
+template <typename T>
+struct Selects<MaxFast<T>> : Selects<Max<T>> {};
+template <>
+struct Selects<MinFast<float>> {
+  static __device__ __forceinline__ bool apply(float acc, float t) { return t < acc; }
+};
+template <>
+struct Selects<MaxFast<float>> {
+  static __device__ __forceinline__ bool apply(float acc, float t) { return acc < t; }
+};
+
 // ---- packed pairs (half) -------------------------------------------------------------------------
 // HADD2 / HMUL2 do two IEEE round-to-nearest half operations per instruction, each half rounded exactly like the
 // scalar __hadd_rn / __hmul_rn; the _rn intrinsics are never contracted into an HFMA2 (a single rounding, which

@@ -189,6 +189,34 @@ MM_API int mm_kernel_enqueue_batched(mm_context *ctx, int dtype, int map_op, int
                                      unsigned size_n, unsigned size_k, unsigned size_m,
                                      unsigned batch, void *cuda_stream);
 
+/* ---- witnesses: which k each element of a Min / Max product came from ---------------------------
+ * mm_kernel_enqueue_witness() computes C exactly as mm_kernel_enqueue_batched() does with the same arguments
+ * (BIT-IDENTICAL for every type, map, flag and tuning value, the float default FMNMX included), and beside it
+ * W[N x M] (uint32, row-major, packed per problem like C).  W[n,m] is the last k at which the sequential reduction
+ * of Naive<> SELECTED its new term t = Map(a[n,k], b[k,m]), with acc the running value:
+ *   literal Min `(acc < t) ? acc : t` (every type; float under MM_FLAG_EXACT): selects t when !(acc < t);
+ *   literal Max `(t < acc) ? acc : t`: selects t when !(t < acc);
+ *     so ties go to the LATEST k, and a NaN term is selected;
+ *   FMNMX Min (float without MM_FLAG_EXACT): selects t when t < acc;  FMNMX Max: when acc < t;
+ *     so ties go to the EARLIEST k, and a NaN term is never selected;
+ * or MM_WITNESS_NONE if no term was ever selected.  Consequences:
+ *   - literal path, W != NONE: C has the bits of term W (any NaN payload);
+ *   - FMNMX path, W != NONE: C equals term W as a number (C may be -0 where term W is +0, and the reverse, as
+ *     documented for MM_FLAG_EXACT);
+ *   - W == NONE: C has the bits of the reduce's identity.  A float Max whose terms all lie below FLT_MIN (the
+ *     reference's identity numeric_limits<float>::min()) gives NONE, as does an FMNMX Min whose terms all equal FLT_MAX.
+ * k counts within the problem: 0 <= W < K whatever the batch index, and with or without MM_FLAG_TRANSPOSED_A.
+ * MM_FLAG_BATCH_SHARED_A / _B work as in batched calls; MM_FLAG_TF32X3 is ignored.
+ * Validation as mm_kernel_enqueue_batched(), plus: w_device NULL or not 16-byte aligned -> MM_ERR_INVALID;
+ * reduce_op other than MM_OP_MIN / MM_OP_MAX -> MM_ERR_INVALID.  W must not overlap A, B or C.  The call uses no
+ * scratch, so it can be captured into a CUDA graph without a reserve; per-call profiling records it like a
+ * semiring call (no preparation time, the whole call is main time).  Callers detect the feature by this symbol. */
+#define MM_WITNESS_NONE 0xFFFFFFFFu
+MM_API int mm_kernel_enqueue_witness(mm_context *ctx, int dtype, int map_op, int reduce_op, int flags,
+                                     const void *a_device, const void *b_device, void *c_device,
+                                     unsigned *w_device, unsigned size_n, unsigned size_k, unsigned size_m,
+                                     unsigned batch, void *cuda_stream);
+
 /* Per-phase device timing of enqueued work, for roofline accounting.  With profiling on, every
  * mm_kernel_enqueue()/mm_kernel_execute() records CUDA events on the launching stream around
  * (i) the operand-preparation kernels and (ii) the main compute kernel.  mm_context_profile_read()

@@ -129,6 +129,51 @@ for case in BATCHED:
             ctx.free(p)
     print("%-42s %s" % (name, "ok" if ok else "MISMATCH"), flush=True)
     bad += 0 if ok else 1
+# witnesses (mm_kernel_enqueue_witness): ragged shapes on both witness kernels, a batch with a shared operand; C must
+# equal the plain batched call and W the test suite's restatement (tests/witness_naive.py).  These cases have run on
+# an H100 without compute-sanitizer so far; no memcheck / racecheck / synccheck pass over them has been made yet.
+import witness_naive  # noqa: E402
+
+WITNESS = [
+    ("witness ring f32 addmin", G.FLOAT, G.ADD, G.MIN, 0, (129, 48, 144), 1),
+    ("witness ring i32 addmax shared B", G.INT32, G.ADD, G.MAX, G.FLAG_BATCH_SHARED_B, (65, 32, 48), 3),
+    ("witness staged f32 exact addmin", G.FLOAT, G.ADD, G.MIN, G.FLAG_EXACT, (129, 48, 144), 1, dict(semiring_ring=0)),
+    ("witness staged f64 addmax TA", G.DOUBLE, G.ADD, G.MAX, G.FLAG_TRANSPOSED_A, (67, 16, 72), 2),
+    ("witness staged u8 maxmin", G.UINT8, G.MAX, G.MIN, 0, (65, 128, 192), 1),
+    ("witness staged bf16 addmax", G.BFLOAT16, G.ADD, G.MAX, 0, (65, 64, 96), 1),
+]
+for case in WITNESS:
+    name, dt, mp, rd, flags, (n, k, m), batch = case[:7]
+    tuning = case[7] if len(case) > 7 else {}
+    if only and only not in name:
+        continue
+    shared_b = bool(flags & G.FLAG_BATCH_SHARED_B)
+    data = [bf16_naive.fill(O, n, k, m, 50 + i) if dt == G.BFLOAT16 else O.fill(dt, n, k, m, 50 + i) for i in range(batch)]
+    ta = bool(flags & G.FLAG_TRANSPOSED_A)
+    a = np.concatenate([(np.ascontiguousarray(d[0].reshape(n, k).T) if ta else d[0]).reshape(-1) for d in data])
+    b = np.concatenate([d[1].reshape(-1) for d in data[:1 if shared_b else batch]])
+    with G.Context(0) as ctx:
+        ctx.set_tuning(**tuning)
+        da, db = ctx.alloc(a.nbytes), ctx.alloc(b.nbytes)
+        dc, dp, dw = (ctx.alloc(batch * n * m * x) for x in (a.itemsize, a.itemsize, 4))
+        ctx.copy_to_device(da, a)
+        ctx.copy_to_device(db, b)
+        ctx.enqueue_batched(dt, mp, rd, da, db, dp, n, k, m, batch, flags=flags)
+        ctx.enqueue_witness(dt, mp, rd, da, db, dc, dw, n, k, m, batch=batch, flags=flags)
+        c, p = np.empty(batch * n * m, dtype=a.dtype), np.empty(batch * n * m, dtype=a.dtype)
+        w = np.empty((batch, n, m), dtype=np.uint32)
+        for host, dev in ((c, dc), (p, dp), (w, dw)):
+            ctx.copy_to_host(host, dev)
+        for x in (da, db, dc, dp, dw):
+            ctx.free(x)
+    ok = c.tobytes() == p.tobytes()
+    fm = dt == G.FLOAT and not flags & G.FLAG_EXACT
+    for i in range(batch):
+        want = witness_naive.witness(dt, mp, rd, data[i][0].reshape(n, k), data[0 if shared_b else i][1].reshape(k, m),
+                                     fmnmx=fm)[1]
+        ok = ok and np.array_equal(w[i], want)
+    print("%-42s %s" % (name, "ok" if ok else "MISMATCH"), flush=True)
+    bad += 0 if ok else 1
 # the row-block split on one device listed twice: sliced upload of B, the gather kernel, host barriers
 if not only or "multi" in only:
     for dt, shape in ((G.FLOAT, (300, 128, 272)), (G.HALF, (257, 128, 288)), (G.DOUBLE, (130, 128, 136)),
