@@ -51,9 +51,9 @@ EXPORTS = ["mm_last_error", "mm_version", "mm_dtype_size", "mm_memory_width", "m
            "mm_kernel_path", "mm_gemm_host", "mm_context_set_profiling", "mm_context_profile_read",
            "mm_context_set_tuning", "mm_context_get_tuning", "mm_context_reserve",
            "mm_kernel_enqueue_batched", "mm_context_reserve_batched", "mm_kernel_enqueue_witness",
-           "mm_multi_create", "mm_multi_destroy", "mm_multi_device_count", "mm_multi_context",
-           "mm_multi_peer_access", "mm_multi_partition", "mm_multi_gemm_host", "mm_multi_upload", "mm_multi_execute",
-           "mm_multi_download"]
+           "mm_kernel_enqueue_accumulate", "mm_multi_create", "mm_multi_destroy", "mm_multi_device_count",
+           "mm_multi_context", "mm_multi_peer_access", "mm_multi_partition", "mm_multi_gemm_host", "mm_multi_upload",
+           "mm_multi_execute", "mm_multi_download"]
 
 
 class MMError(RuntimeError):
@@ -99,6 +99,7 @@ def lib():
         L.mm_kernel_enqueue_batched.argtypes = [vp, i, i, i, i, vp, vp, vp, u, u, u, u, vp]
         L.mm_context_reserve_batched.argtypes = [vp, i, i, u, u, u, u]
         L.mm_kernel_enqueue_witness.argtypes = [vp, i, i, i, i, vp, vp, vp, vp, u, u, u, u, vp]
+        L.mm_kernel_enqueue_accumulate.argtypes = [vp, i, i, i, i, vp, vp, vp, u, u, u, u, vp]
         L.mm_multi_create.argtypes = [i, ctypes.POINTER(i), ctypes.POINTER(vp)]
         L.mm_multi_destroy.argtypes = [vp]
         L.mm_multi_device_count.argtypes = [vp]
@@ -198,6 +199,13 @@ class Context:
         Max reduce, the k whose term each element of C was selected from last, or WITNESS_NONE (include/mm_b200.h)."""
         _check(lib().mm_kernel_enqueue_witness(self._h, dtype, map_op, reduce_op, flags, a_dev, b_dev, c_dev, w_dev,
                                                n, k, m, batch, ctypes.c_void_p(stream) if stream else None))
+
+    def enqueue_accumulate(self, dtype, map_op, reduce_op, a_dev, b_dev, c_dev, n, k, m, batch=1, flags=0,
+                           stream=None):
+        """C <- R(C, P) in place: P is what enqueue_batched would write with the same arguments, R one application of
+        the call's reduce with the old C first (include/mm_b200.h).  C must not overlap A or B."""
+        _check(lib().mm_kernel_enqueue_accumulate(self._h, dtype, map_op, reduce_op, flags, a_dev, b_dev, c_dev,
+                                                  n, k, m, batch, ctypes.c_void_p(stream) if stream else None))
 
     def set_tuning(self, **knobs):
         """mm_context_set_tuning by name, e.g. ctx.set_tuning(cta_group=1, stages=4)."""

@@ -216,6 +216,12 @@ int check_batch(unsigned batch, unsigned n, unsigned k, unsigned m) {
   return MM_OK;
 }
 
+// Whether the byte ranges [x, x + x_bytes) and [y, y + y_bytes) share a byte.
+bool overlaps(const void *x, size_t x_bytes, const void *y, size_t y_bytes) {
+  const uintptr_t x0 = reinterpret_cast<uintptr_t>(x), y0 = reinterpret_cast<uintptr_t>(y);
+  return x0 < y0 + y_bytes && y0 < x0 + x_bytes;
+}
+
 // Stream-capture and profiling bookkeeping of one enqueued call.  *pe = the call's three profiling events (start,
 // after preparation, after the main kernel; the start one already recorded), or null when `profile` is false or
 // profiling is off or full.
@@ -241,10 +247,11 @@ int begin_call(mm_context *ctx, cudaStream_t stream, bool profile, cudaStreamCap
 
 int enqueue_locked(mm_context *ctx, int dtype, int map_op, int reduce_op, int flags, const void *a,
                    const void *b, void *c, unsigned n, unsigned k, unsigned m, cudaStream_t stream,
-                   bool dry_run = false, unsigned batch = 1) {
+                   bool dry_run = false, unsigned batch = 1, bool accumulate = false) {
   mm::GemmArgs g = make_args(ctx, a, b, c, n, k, m, flags, stream);
   g.batch = make_batch(batch, flags);
   g.dry_run = dry_run;
+  g.accumulate = accumulate;
   cudaStreamCaptureStatus capture;
   cudaEvent_t *pe;
   const int rc_begin = begin_call(ctx, stream, !dry_run, &capture, &pe);
@@ -268,11 +275,12 @@ int enqueue_locked(mm_context *ctx, int dtype, int map_op, int reduce_op, int fl
     }
     case kPathDmma:
       if (pe) MM_CUDA_TRY(cudaEventRecord(pe[1], stream));
-      rc_launch = mm::launch_dmma(g);
+      rc_launch = accumulate ? mm::launch_dmma_accumulate(g) : mm::launch_dmma(g);
       break;
     case kPathSemiring:
       if (pe) MM_CUDA_TRY(cudaEventRecord(pe[1], stream));
-      rc_launch = mm::launch_semiring(dtype, map_op, reduce_op, g);
+      rc_launch = accumulate ? mm::launch_semiring_accumulate(dtype, map_op, reduce_op, g)
+                             : mm::launch_semiring(dtype, map_op, reduce_op, g);
       break;
   }
   if (rc_launch != MM_OK) return rc_launch;
@@ -862,6 +870,28 @@ int mm_kernel_enqueue_batched(mm_context *ctx, int dtype, int map_op, int reduce
   MM_CUDA_TRY(cudaSetDevice(ctx->device));
   cudaStream_t s = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ctx->stream;
   return enqueue_locked(ctx, dtype, map_op, reduce_op, flags, a, b, c, n, k, m, s, /*dry_run=*/false, batch);
+}
+
+int mm_kernel_enqueue_accumulate(mm_context *ctx, int dtype, int map_op, int reduce_op, int flags, const void *a,
+                                 const void *b, void *c, unsigned n, unsigned k, unsigned m, unsigned batch,
+                                 void *cuda_stream) {
+  if (!ctx) return fail(MM_ERR_INVALID, "null context");
+  int rc = check_args(dtype, map_op, reduce_op, a, b, c, n, k, m);
+  if (rc != MM_OK) return rc;
+  if ((rc = check_batch(batch, n, k, m)) != MM_OK) return rc;
+  if ((rc = check_device_alignment(a, b, c)) != MM_OK) return rc;
+  // C is read and written while A and B are read: an overlap would feed updated elements back into the product
+  const size_t es = mm_dtype_size(dtype);
+  const mm::GemmBatch bt = make_batch(batch, flags);
+  if (overlaps(c, size_t(batch) * n * m * es, a, size_t(bt.a_copies()) * n * k * es) ||
+      overlaps(c, size_t(batch) * n * m * es, b, size_t(bt.b_copies()) * k * m * es)) {
+    return fail(MM_ERR_INVALID, "C must not overlap A or B in an accumulating call");
+  }
+  std::lock_guard<std::mutex> lock(ctx->mutex);
+  MM_CUDA_TRY(cudaSetDevice(ctx->device));
+  cudaStream_t s = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ctx->stream;
+  return enqueue_locked(ctx, dtype, map_op, reduce_op, flags, a, b, c, n, k, m, s, /*dry_run=*/false, batch,
+                        /*accumulate=*/true);
 }
 
 int mm_kernel_enqueue_witness(mm_context *ctx, int dtype, int map_op, int reduce_op, int flags, const void *a,

@@ -85,6 +85,8 @@ struct GemmArgs {
   // attributes, which also forces the lazily loaded cubin in).  mm_kernel_execute runs it before
   // recording its start event so that the reported device time is kernel time only.
   bool dry_run = false;
+  // mm_kernel_enqueue_accumulate: C <- Reduce(C_old, product), C_old read in the compute kernel's epilogue
+  bool accumulate = false;
 };
 
 // ---- kernel families (one launcher per translation unit) ---------------------------------------
@@ -92,6 +94,8 @@ struct GemmArgs {
 int launch_semiring(int dtype, int map_op, int reduce_op, const GemmArgs &args);
 // The same C for a Min / Max reduce, plus the witness W (N x M uint32 per problem).  semiring_witness_*.cu
 int launch_semiring_witness(int dtype, int map_op, int reduce_op, const GemmArgs &args, unsigned *w);
+// C <- Reduce(C_old, product) with the same kernel choice as launch_semiring.  semiring_accumulate_*.cu
+int launch_semiring_accumulate(int dtype, int map_op, int reduce_op, const GemmArgs &args);
 
 // wgmma tensor-core GEMM for (Multiply, Add) float (tf32), half (f16) and uint8_t (u8).
 // The context's scratch holds, in this order: [B operand copy][A operand copy][counters].
@@ -155,7 +159,8 @@ int tcgen05_prepare_a(int dtype, const void *a, void *aprep, unsigned rows, unsi
 // producer waits for b_ready[column tile] >= b_ready_target before it fetches a tile's B panel.
 int tcgen05_gemm(int dtype, const void *a_op, const void *b_op, void *c, unsigned rows, unsigned k, unsigned m,
                  int flags, const Tuning &t, unsigned int *tile_sync, const unsigned int *b_ready,
-                 unsigned b_ready_target, cudaStream_t stream, const GemmBatch &batch = GemmBatch{});
+                 unsigned b_ready_target, cudaStream_t stream, const GemmBatch &batch = GemmBatch{},
+                 bool accumulate = false);
 constexpr size_t kTcgen05TailBytes = 256 + 64 * 1024;  // [panel counters, 64 KiB][wave-barrier counter, 256 B]
 // Generic gather of row-sliced B into one local array (identity transform): what the multi-GPU path
 // uses for the kernel families that read B as is (double, semirings, half).
@@ -163,5 +168,7 @@ int gather_b_rows(const BSource &src, void *dst, size_t elem_bytes, unsigned k, 
 
 // DMMA (mma.sync m8n8k4 f64) GEMM for (Multiply, Add) double.  gemm_dmma.cu
 int launch_dmma(const GemmArgs &args);
+// The same with C <- C_old + product.  gemm_dmma_acc.cu
+int launch_dmma_accumulate(const GemmArgs &args);
 
 }  // namespace mm

@@ -30,7 +30,7 @@
 //     half, so it shares half's transpose kernel.
 //
 // The GEMM kernel and its launcher are in gemm_wgmma.cuh.  This unit instantiates them for tf32, f16 and
-// u8; the bf16 instantiations are in gemm_wgmma_bf16.cu.
+// u8; the bf16 instantiations are in gemm_wgmma_bf16.cu, the accumulate kernels in gemm_wgmma_acc.cu.
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -453,7 +453,13 @@ int tcgen05_prepare_a(int dtype, const void *a, void *aprep, unsigned rows, unsi
 namespace {
 int gemm_dispatch(int dtype, const void *a_op, const void *b_op, void *c, unsigned rows, unsigned k, unsigned m,
                   int flags, const Tuning &t, unsigned int *tile_sync, const unsigned int *b_ready,
-                  unsigned b_ready_target, bool attributes_only, cudaStream_t stream, const GemmBatch &batch) {
+                  unsigned b_ready_target, bool attributes_only, cudaStream_t stream, const GemmBatch &batch,
+                  bool accumulate = false) {
+  if (accumulate) {
+    if (split3(dtype, flags)) k *= 3;
+    return wgmma_accumulate_gemm(dtype, a_op, b_op, c, rows, k, m, t, tile_sync, b_ready, b_ready_target,
+                                 attributes_only, stream, batch);
+  }
   if (dtype == MM_DTYPE_BFLOAT16) {
     return wgmma_bf16_gemm(a_op, b_op, c, rows, k, m, t, tile_sync, b_ready, b_ready_target, attributes_only, stream,
                            batch);
@@ -472,12 +478,13 @@ int gemm_dispatch(int dtype, const void *a_op, const void *b_op, void *c, unsign
 
 }  // namespace
 
-// C[rows x m] = Aop[rows x k] * B on the tensor cores; `b_op` as returned by tcgen05_prepare_b.
+// C[rows x m] = Aop[rows x k] * B on the tensor cores; `b_op` as returned by tcgen05_prepare_b.  `accumulate`:
+// C <- C + that product, by the accumulate kernels.
 int tcgen05_gemm(int dtype, const void *a_op, const void *b_op, void *c, unsigned rows, unsigned k, unsigned m,
                  int flags, const Tuning &t, unsigned int *tile_sync, const unsigned int *b_ready,
-                 unsigned b_ready_target, cudaStream_t stream, const GemmBatch &batch) {
+                 unsigned b_ready_target, cudaStream_t stream, const GemmBatch &batch, bool accumulate) {
   return gemm_dispatch(dtype, a_op, b_op, c, rows, k, m, flags, t, tile_sync, b_ready, b_ready_target, false, stream,
-                       batch);
+                       batch, accumulate);
 }
 
 int tcgen05_prepare_b_async(int dtype, const BSource &src, void *local_b, void *scratch, size_t scratch_bytes,
@@ -551,7 +558,7 @@ int launch_tcgen05(int dtype, const GemmArgs &g, void *scratch, size_t scratch_b
   if (rc == MM_OK && g.ev_prep_done) cudaEventRecord(g.ev_prep_done, g.stream);
   if (rc == MM_OK) {
     rc = tcgen05_gemm(dtype, a_op, pb.b_op, g.c, g.n, g.k, g.m, g.flags, t, cnt.tile_sync, pb.ready, pb.ready_target,
-                      g.stream, g.batch);
+                      g.stream, g.batch, g.accumulate);
   }
   if (pb.forked) cudaStreamWaitEvent(g.stream, g.ev_join, 0);  // join, on the error paths too
   return rc;

@@ -1,6 +1,7 @@
 // The wgmma tensor-core GEMM kernel (C = A' * B'^T, both operands K-major) and its host-side launch
 // machinery: tensor maps, run-time parameters and the per-variant launcher.  Shared by the translation
-// units that instantiate it: gemm_tcgen05.cu (tf32, f16, u8) and gemm_wgmma_bf16.cu (bf16).  The kernel's
+// units that instantiate it: gemm_tcgen05.cu (tf32, f16, u8), gemm_wgmma_bf16.cu (bf16) and gemm_wgmma_acc.cu (the
+// accumulate kernels of every type).  The kernel's
 // structure is described at the top of gemm_tcgen05.cu.
 #pragma once
 
@@ -68,20 +69,42 @@ __device__ __forceinline__ TileCoord tile_coord(uint32_t t, uint32_t tiles_r, ui
 }
 
 // ---- epilogue ------------------------------------------------------------------------------------
-// Two adjacent accumulator values (columns c, c + 1 of one row) as the bytes of C.
+// Two adjacent accumulator values (columns c, c + 1 of one row) as the bytes of C.  The accumulate kernel
+// (mm_kernel_enqueue_accumulate) then combines them with the old pair of C: add(old, p) = C_old + P, elementwise,
+// in the type of C and with C_old as the first operand (load: ld.global, coherent with the kernel's own stores).
 template <typename TOut>
 struct Pair;
 template <>
 struct Pair<float> {
   using T = uint2;
   __device__ __forceinline__ static uint2 make(uint32_t a, uint32_t b) { return make_uint2(a, b); }
+  __device__ __forceinline__ static uint2 load(const uint2 *p) {
+    uint2 v;
+    asm volatile("ld.global.v2.b32 {%0, %1}, [%2];" : "=r"(v.x), "=r"(v.y) : "l"(p));
+    return v;
+  }
+  __device__ __forceinline__ static uint2 add(uint2 old, uint2 p) {
+    return make_uint2(__float_as_uint(__fadd_rn(__uint_as_float(old.x), __uint_as_float(p.x))),
+                      __float_as_uint(__fadd_rn(__uint_as_float(old.y), __uint_as_float(p.y))));
+  }
 };
+__device__ __forceinline__ uint32_t ld_global_b32(const uint32_t *p) {
+  uint32_t v;
+  asm volatile("ld.global.b32 %0, [%1];" : "=r"(v) : "l"(p));
+  return v;
+}
 template <>
 struct Pair<__half> {
   using T = uint32_t;
   __device__ __forceinline__ static uint32_t make(uint32_t a, uint32_t b) {
     __half2 h = __floats2half2_rn(__uint_as_float(a), __uint_as_float(b));
     return *reinterpret_cast<uint32_t *>(&h);
+  }
+  __device__ __forceinline__ static uint32_t load(const uint32_t *p) { return ld_global_b32(p); }
+  // HADD2: each half rounded exactly like the scalar __hadd_rn
+  __device__ __forceinline__ static uint32_t add(uint32_t old, uint32_t p) {
+    __half2 s = __hadd2_rn(*reinterpret_cast<__half2 *>(&old), *reinterpret_cast<__half2 *>(&p));
+    return *reinterpret_cast<uint32_t *>(&s);
   }
 };
 // bfloat16: both accumulators rounded to nearest by one cvt.rn.bf16x2.f32.
@@ -92,6 +115,11 @@ struct Pair<__nv_bfloat16> {
     __nv_bfloat162 h = __floats2bfloat162_rn(__uint_as_float(a), __uint_as_float(b));
     return *reinterpret_cast<uint32_t *>(&h);
   }
+  __device__ __forceinline__ static uint32_t load(const uint32_t *p) { return ld_global_b32(p); }
+  __device__ __forceinline__ static uint32_t add(uint32_t old, uint32_t p) {
+    __nv_bfloat162 s = __hadd2_rn(*reinterpret_cast<__nv_bfloat162 *>(&old), *reinterpret_cast<__nv_bfloat162 *>(&p));
+    return *reinterpret_cast<uint32_t *>(&s);
+  }
 };
 // uint8_t: the accumulator is the exact 32-bit sum; its low byte is the reference's result (arithmetic modulo 256).
 template <>
@@ -99,6 +127,17 @@ struct Pair<unsigned char> {
   using T = unsigned short;
   __device__ __forceinline__ static unsigned short make(uint32_t a, uint32_t b) {
     return static_cast<unsigned short>((a & 0xFFu) | ((b & 0xFFu) << 8));
+  }
+  __device__ __forceinline__ static unsigned short load(const unsigned short *p) {
+    unsigned short v;
+    asm volatile("ld.global.b16 %0, [%1];" : "=h"(v) : "l"(p));
+    return v;
+  }
+  // two bytes, each added modulo 256
+  __device__ __forceinline__ static unsigned short add(unsigned short old, unsigned short p) {
+    const uint32_t lo = (uint32_t(old) + uint32_t(p)) & 0xFFu;
+    const uint32_t hi = ((uint32_t(old) >> 8) + (uint32_t(p) >> 8)) & 0xFFu;
+    return static_cast<unsigned short>(lo | (hi << 8));
   }
 };
 
@@ -144,11 +183,11 @@ struct GemmParams {
 };
 
 // C[rows x cols] = A'[rows x k] * B'^T ; A' (rows x k) and B' (cols x k) K-major.  CG == 2 must be
-// launched with cluster dimension (2, 1, 1).
-template <int KIND, typename TOut, int CG, int BN>
-__global__ void __launch_bounds__(NUM_THREADS, 1)
-gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-                  const __grid_constant__ CUtensorMap tmap_c, TOut *__restrict__ C, const GemmParams p) {
+// launched with cluster dimension (2, 1, 1).  ACC: C = C_old + A'B'^T, the add applied to the rounded product in
+// the epilogue (gemm_wgmma_accumulate_kernel); nothing else differs.
+template <int KIND, typename TOut, int CG, int BN, bool ACC>
+__device__ __forceinline__ void gemm_wgmma_body(const CUtensorMap &tmap_a, const CUtensorMap &tmap_b,
+                                                const CUtensorMap &tmap_c, TOut *__restrict__ C, const GemmParams &p) {
   using G = Geo<CG, BN>;
   constexpr int ELEM_BYTES = (KIND == ptx::KIND_TF32) ? 4 : (KIND == ptx::KIND_I8 ? 1 : 2);  // f16, bf16: 2
   constexpr int BLOCK_K_ELEMS = BLOCK_K_BYTES / ELEM_BYTES;
@@ -292,6 +331,23 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
         for (int chunk = 0; chunk < BN / 32; ++chunk) {
           const uint32_t col = tc.c * BN + chunk * 32;
           if (row0 < rows && col < cols) {                        // warp-uniform
+            typename P::T old[4][2];
+            if constexpr (ACC) {
+              // C_old of this lane's pairs, all eight loads in flight before the first is used; pairs outside
+              // the problem are not read (the TMA store clips them)
+              const TOut *Cp = C + size_t(tc.prob) * rows * cols;
+#pragma unroll
+              for (int j = 0; j < 4; ++j) {
+#pragma unroll
+                for (int i = 0; i < 2; ++i) {
+                  const uint32_t row = row0 + r_in + 8 * i, c = col + 8 * j + c_in;
+                  old[j][i] = typename P::T{};
+                  if (row < rows && c < cols) {
+                    old[j][i] = P::load(reinterpret_cast<const typename P::T *>(Cp + size_t(row) * cols + c));
+                  }
+                }
+              }
+            }
             if (lane == 0) ptx::tma_store_wait_read<0>();         // the previous block has left the buffer
             __syncwarp();
 #pragma unroll
@@ -300,7 +356,9 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
               for (int i = 0; i < 2; ++i) {
                 const uint32_t a = buf + (r_in + 8 * i) * PITCH + (8 * j + c_in) * sizeof(TOut);
                 const int reg = 4 * (4 * chunk + j) + 2 * i;
-                st_shared_pair(a ^ (((a >> 7) & SW_MASK) << 4), P::make(acc[reg], acc[reg + 1]));
+                typename P::T v = P::make(acc[reg], acc[reg + 1]);
+                if constexpr (ACC) v = P::add(old[j][i], v);
+                st_shared_pair(a ^ (((a >> 7) & SW_MASK) << 4), v);
               }
             }
             ptx::fence_proxy_async_smem();                        // generic-proxy smem writes -> TMA read
@@ -319,10 +377,30 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
           const uint32_t row = row0 + r_in + 8 * i;
           if (row >= rows) continue;
           typename P::T *crow = reinterpret_cast<typename P::T *>(Cp + size_t(row) * cols);
+          if constexpr (ACC) {
+            // groups of eight pairs: eight loads of C_old in flight, then eight stores
 #pragma unroll
-          for (int j = 0; j < BN / 8; ++j) {
-            const uint32_t col = tc.c * BN + 8 * j + c_in;
-            if (col < cols) crow[col / 2] = P::make(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]);
+            for (int j0 = 0; j0 < BN / 8; j0 += 8) {
+              typename P::T old[8];
+#pragma unroll
+              for (int j = 0; j < 8; ++j) {
+                const uint32_t col = tc.c * BN + 8 * (j0 + j) + c_in;
+                old[j] = typename P::T{};
+                if (col < cols) old[j] = P::load(crow + col / 2);
+              }
+#pragma unroll
+              for (int j = 0; j < 8; ++j) {
+                const uint32_t col = tc.c * BN + 8 * (j0 + j) + c_in;
+                const int reg = 4 * (j0 + j) + 2 * i;
+                if (col < cols) crow[col / 2] = P::add(old[j], P::make(acc[reg], acc[reg + 1]));
+              }
+            }
+          } else {
+#pragma unroll
+            for (int j = 0; j < BN / 8; ++j) {
+              const uint32_t col = tc.c * BN + 8 * j + c_in;
+              if (col < cols) crow[col / 2] = P::make(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]);
+            }
           }
         }
       }
@@ -332,6 +410,21 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
 
   // no CTA of a cluster leaves while its peer may still multicast into it or arrive on its barriers
   if (CG == 2) cluster_sync_all();
+}
+
+template <int KIND, typename TOut, int CG, int BN>
+__global__ void __launch_bounds__(NUM_THREADS, 1)
+gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                  const __grid_constant__ CUtensorMap tmap_c, TOut *__restrict__ C, const GemmParams p) {
+  gemm_wgmma_body<KIND, TOut, CG, BN, false>(tmap_a, tmap_b, tmap_c, C, p);
+}
+
+// C <- C + A'B'^T (mm_kernel_enqueue_accumulate); instantiated in gemm_wgmma_acc.cu only.
+template <int KIND, typename TOut, int CG, int BN>
+__global__ void __launch_bounds__(NUM_THREADS, 1)
+gemm_wgmma_accumulate_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                             const __grid_constant__ CUtensorMap tmap_c, TOut *__restrict__ C, const GemmParams p) {
+  gemm_wgmma_body<KIND, TOut, CG, BN, true>(tmap_a, tmap_b, tmap_c, C, p);
 }
 
 // ---- host side -----------------------------------------------------------------------------------
@@ -404,10 +497,17 @@ struct LaunchPlan {
   cudaStream_t stream;
 };
 
-template <int KIND, typename TOut, int CG, int BN>
+// Only the kernel a translation unit launches is instantiated there.
+template <int KIND, typename TOut, int CG, int BN, bool ACC>
+constexpr auto gemm_kernel_ptr() {
+  if constexpr (ACC) return gemm_wgmma_accumulate_kernel<KIND, TOut, CG, BN>;
+  else return gemm_wgmma_kernel<KIND, TOut, CG, BN>;
+}
+
+template <int KIND, typename TOut, int CG, int BN, bool ACC>
 int launch_gemm_variant(LaunchPlan plan) {
   using G = Geo<CG, BN>;
-  auto kern = gemm_wgmma_kernel<KIND, TOut, CG, BN>;
+  auto kern = gemm_kernel_ptr<KIND, TOut, CG, BN, ACC>();
   // Ring depth: the deepest that fits unless the tuning asks for less.
   const int stages = plan.requested_stages <= 0 ? G::MAX_STAGES
                                                  : std::min(std::max(plan.requested_stages, 2), int(G::MAX_STAGES));
@@ -435,10 +535,11 @@ int launch_gemm_variant(LaunchPlan plan) {
   return MM_OK;
 }
 
-template <int KIND, typename TOut>
+// ACC: the accumulate kernels (gemm_wgmma_acc.cu)
+template <int KIND, typename TOut, bool ACC = false>
 int dispatch_variant(int cg, int bn, const LaunchPlan &plan) {
 #define MM_VARIANT(CGV, BNV) \
-  if (cg == CGV && bn == BNV) return launch_gemm_variant<KIND, TOut, CGV, BNV>(plan);
+  if (cg == CGV && bn == BNV) return launch_gemm_variant<KIND, TOut, CGV, BNV, ACC>(plan);
   MM_VARIANT(2, 256)
   MM_VARIANT(1, 256)
   MM_VARIANT(2, 128)
@@ -492,5 +593,11 @@ int plan_gemm(int dtype, const void *a_op, const void *b_op, void *c, unsigned r
 int wgmma_bf16_gemm(const void *a_op, const void *b_op, void *c, unsigned rows, unsigned k, unsigned m, const Tuning &t,
                     unsigned int *tile_sync, const unsigned int *b_ready, unsigned b_ready_target, bool attributes_only,
                     cudaStream_t stream, const GemmBatch &batch);
+
+// C <- C + product for every type of the wgmma path (mm_kernel_enqueue_accumulate): the sixteen accumulate kernels
+// live in gemm_wgmma_acc.cu.  `k` is the K extent the operands carry (3K for 3xTF32).
+int wgmma_accumulate_gemm(int dtype, const void *a_op, const void *b_op, void *c, unsigned rows, unsigned k, unsigned m,
+                          const Tuning &t, unsigned int *tile_sync, const unsigned int *b_ready,
+                          unsigned b_ready_target, bool attributes_only, cudaStream_t stream, const GemmBatch &batch);
 
 }  // namespace mm

@@ -81,15 +81,13 @@ struct SemiringBf162 {
       std::is_same<T, __nv_bfloat16>::value && PackedOpB<Map>::value && PackedOpB<Reduce>::value;
 };
 
-// 2 CTAs (16 warps) per SM for 4-byte element types and packed half / bfloat16: 64 accumulators + two k-steps of fragments fit
-// in 128 registers without spilling.  8-byte types need the full 255-register budget, and unpacked 1- and
-// 2-byte types (one 32-bit register per element) spill at 128: those run 1 CTA per SM.
-template <typename T, class Map, class Reduce>
-__global__ void __launch_bounds__(256, (sizeof(T) == 4 || SemiringHalf2<T, Map, Reduce>::value ||
-                                       SemiringBf162<T, Map, Reduce>::value) ? 2 : 1)
-semiring_tile_kernel(const T *__restrict__ A, const __grid_constant__ CUtensorMap tmap_b, T *__restrict__ C,
-                     unsigned size_n, unsigned size_k, unsigned size_m,
-                     bool TRANSPOSED_A, unsigned a_step, unsigned b_step) {
+// ACC: C = Reduce(C_old, result), applied in the epilogue to the old C at the addresses about to be stored
+// (semiring_accumulate_tile_kernel); nothing else differs.
+template <typename T, class Map, class Reduce, bool ACC>
+__device__ __forceinline__ void semiring_tile_body(const T *__restrict__ A, const CUtensorMap &tmap_b,
+                                                   T *__restrict__ C, unsigned size_n, unsigned size_k,
+                                                   unsigned size_m, bool TRANSPOSED_A, unsigned a_step,
+                                                   unsigned b_step) {
   using Cfg = SemiringTile<T>;
   constexpr int BM = Cfg::BM, BN = Cfg::BN, BK = Cfg::BK, VEC = Cfg::VEC;
   constexpr int LDA = Cfg::LDA, LDB = Cfg::LDB;
@@ -279,10 +277,46 @@ semiring_tile_kernel(const T *__restrict__ A, const __grid_constant__ CUtensorMa
             out.v[q] = acc[i][h * 4 + q];
           }
         }
+        if constexpr (ACC) {
+          const Quad<T> old = *reinterpret_cast<const Quad<T> *>(C + row * size_m + col);
+#pragma unroll
+          for (int p = 0; p < 4; p += 2) {
+            if constexpr (kHalf2) {
+              const T2 r = ReduceOp2::Apply2(P2::pair(old.v[p], old.v[p + 1]), P2::pair(out.v[p], out.v[p + 1]));
+              out.v[p] = P2::lo(r);
+              out.v[p + 1] = P2::hi(r);
+            } else {
+              out.v[p] = Reduce::Apply(old.v[p], out.v[p]);
+              out.v[p + 1] = Reduce::Apply(old.v[p + 1], out.v[p + 1]);
+            }
+          }
+        }
         *reinterpret_cast<Quad<T> *>(C + row * size_m + col) = out;
       }
     }
   }
+}
+
+// 2 CTAs (16 warps) per SM for 4-byte element types and packed half / bfloat16: 64 accumulators + two k-steps of fragments fit
+// in 128 registers without spilling.  8-byte types need the full 255-register budget, and unpacked 1- and
+// 2-byte types (one 32-bit register per element) spill at 128: those run 1 CTA per SM.
+template <typename T, class Map, class Reduce>
+__global__ void __launch_bounds__(256, (sizeof(T) == 4 || SemiringHalf2<T, Map, Reduce>::value ||
+                                       SemiringBf162<T, Map, Reduce>::value) ? 2 : 1)
+semiring_tile_kernel(const T *__restrict__ A, const __grid_constant__ CUtensorMap tmap_b, T *__restrict__ C,
+                     unsigned size_n, unsigned size_k, unsigned size_m,
+                     bool TRANSPOSED_A, unsigned a_step, unsigned b_step) {
+  semiring_tile_body<T, Map, Reduce, false>(A, tmap_b, C, size_n, size_k, size_m, TRANSPOSED_A, a_step, b_step);
+}
+
+// C <- Reduce(C_old, A (x) B) (mm_kernel_enqueue_accumulate); instantiated by semiring_accumulate_inst.cu only.
+template <typename T, class Map, class Reduce>
+__global__ void __launch_bounds__(256, (sizeof(T) == 4 || SemiringHalf2<T, Map, Reduce>::value ||
+                                       SemiringBf162<T, Map, Reduce>::value) ? 2 : 1)
+semiring_accumulate_tile_kernel(const T *__restrict__ A, const __grid_constant__ CUtensorMap tmap_b,
+                                T *__restrict__ C, unsigned size_n, unsigned size_k, unsigned size_m,
+                                bool TRANSPOSED_A, unsigned a_step, unsigned b_step) {
+  semiring_tile_body<T, Map, Reduce, true>(A, tmap_b, C, size_n, size_k, size_m, TRANSPOSED_A, a_step, b_step);
 }
 
 }  // namespace mm
@@ -291,7 +325,15 @@ semiring_tile_kernel(const T *__restrict__ A, const __grid_constant__ CUtensorMa
 
 namespace mm {
 
-template <typename T, class Map, class Reduce>
+// Only the kernels a translation unit launches are instantiated there.
+template <typename T, class Map, class Reduce, bool ACC>
+constexpr auto semiring_tile_kernel_ptr() {
+  if constexpr (ACC) return semiring_accumulate_tile_kernel<T, Map, Reduce>;
+  else return semiring_tile_kernel<T, Map, Reduce>;
+}
+
+// ACC: the accumulate kernels, with the same choice between the ring and the tile kernel.
+template <typename T, class Map, class Reduce, bool ACC = false>
 int launch_semiring_typed(const void *a, const void *b, void *c, unsigned n, unsigned k, unsigned m,
                           bool transposed_a, bool ring, const GemmBatch &batch, cudaStream_t stream) {
   using Cfg = SemiringTile<T>;
@@ -299,13 +341,13 @@ int launch_semiring_typed(const void *a, const void *b, void *c, unsigned n, uns
     // 4-byte types with A stored row-major take the ring variant (both tiles by TMA, no block-wide barrier:
     // 41.7 vs 39.9 TOp/s for float (Add, Min) at 8192^3); the tuning knob MM_TUNE_SEMIRING_RING = 0 keeps this kernel
     if (ring && !transposed_a && (a == nullptr || reinterpret_cast<uintptr_t>(a) % 16 == 0)) {
-      return launch_semiring_ring<T, Map, Reduce>(a, b, c, n, k, m, batch.count, batch.shared_a, batch.shared_b,
-                                                  stream);
+      return launch_semiring_ring<T, Map, Reduce, ACC>(a, b, c, n, k, m, batch.count, batch.shared_a, batch.shared_b,
+                                                       stream);
     }
   }
   if (a == nullptr) {  // dry run: only make sure the kernel is loaded
     cudaFuncAttributes attr;
-    return static_cast<int>(cudaFuncGetAttributes(&attr, semiring_tile_kernel<T, Map, Reduce>));
+    return static_cast<int>(cudaFuncGetAttributes(&attr, semiring_tile_kernel_ptr<T, Map, Reduce, ACC>()));
   }
   dim3 grid((m + Cfg::BN - 1) / Cfg::BN, (n + Cfg::BM - 1) / Cfg::BM, batch.count);
   dim3 block(Cfg::THREADS);
@@ -317,7 +359,7 @@ int launch_semiring_typed(const void *a, const void *b, void *c, unsigned n, uns
   if (encode_plain_2d(&tmap_b, b, sizeof(T), b_rows, m, Cfg::BK, Cfg::BN) != 0) {
     return static_cast<int>(cudaErrorInvalidValue);
   }
-  semiring_tile_kernel<T, Map, Reduce><<<grid, block, Cfg::SMEM_BYTES, stream>>>(
+  semiring_tile_kernel_ptr<T, Map, Reduce, ACC>()<<<grid, block, Cfg::SMEM_BYTES, stream>>>(
       pa, tmap_b, pc, n, k, m, transposed_a, batch.shared_a ? 0u : 1u, batch.shared_b ? 0u : 1u);
   return static_cast<int>(cudaGetLastError());
 }
@@ -329,18 +371,24 @@ template <typename T, int MAP_OP>
 int launch_semiring_for(int reduce_op, const void *a, const void *b, void *c, unsigned n, unsigned k,
                         unsigned m, bool ta, bool ring, const GemmBatch &batch, cudaStream_t stream);
 
+// The same for the accumulate kernels (semiring_accumulate_inst.cu).
+template <typename T, int MAP_OP>
+int launch_semiring_accumulate_for(int reduce_op, const void *a, const void *b, void *c, unsigned n, unsigned k,
+                                   unsigned m, bool ta, bool ring, const GemmBatch &batch, cudaStream_t stream);
+
 #define MM_SEMIRING_CASE(REDOP)                                                                    \
   if (reduce_op == REDOP)                                                                          \
     return launch_semiring_typed<T, typename OpSelect<T, MAP_OP>::type,                            \
-                                 typename OpSelect<T, REDOP>::type>(a, b, c, n, k, m, ta, ring, batch, stream);
+                                 typename OpSelect<T, REDOP>::type, ACC>(a, b, c, n, k, m, ta, ring, batch, stream);
 
-#define MM_INSTANTIATE_SEMIRING(TYPE, MAPOP)                                                       \
+#define MM_INSTANTIATE_SEMIRING_FN(FN, ACCV, TYPE, MAPOP)                                          \
   template <>                                                                                      \
-  int launch_semiring_for<TYPE, MAPOP>(int reduce_op, const void *a, const void *b, void *c,       \
-                                       unsigned n, unsigned k, unsigned m, bool ta, bool ring,     \
-                                       const GemmBatch &batch, cudaStream_t stream) {          \
+  int FN<TYPE, MAPOP>(int reduce_op, const void *a, const void *b, void *c,                        \
+                      unsigned n, unsigned k, unsigned m, bool ta, bool ring,                      \
+                      const GemmBatch &batch, cudaStream_t stream) {                               \
     using T = TYPE;                                                                                \
     constexpr int MAP_OP = MAPOP;                                                                  \
+    constexpr bool ACC = ACCV;                                                                     \
     MM_SEMIRING_CASE(MM_OP_MULTIPLY)                                                               \
     MM_SEMIRING_CASE(MM_OP_ADD)                                                                    \
     MM_SEMIRING_CASE(MM_OP_MIN)                                                                    \
@@ -352,5 +400,8 @@ int launch_semiring_for(int reduce_op, const void *a, const void *b, void *c, un
     }                                                                                              \
     return -1;                                                                                     \
   }
+#define MM_INSTANTIATE_SEMIRING(TYPE, MAPOP) MM_INSTANTIATE_SEMIRING_FN(launch_semiring_for, false, TYPE, MAPOP)
+#define MM_INSTANTIATE_SEMIRING_ACCUMULATE(TYPE, MAPOP) \
+  MM_INSTANTIATE_SEMIRING_FN(launch_semiring_accumulate_for, true, TYPE, MAPOP)
 
 }  // namespace mm

@@ -35,11 +35,11 @@ struct SemiringRing {
   static constexpr size_t SMEM_BYTES = size_t(STAGES) * STAGE_BYTES + 2 * STAGES * 8 + 1024;
 };
 
-template <typename T, class Map, class Reduce>
-__global__ void __launch_bounds__(256, 2)
-semiring_ring_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-                     T *__restrict__ C, unsigned size_n, unsigned size_k, unsigned size_m, unsigned a_step,
-                     unsigned b_step) {
+// ACC: C = Reduce(C_old, result) in the epilogue (semiring_accumulate_ring_kernel).
+template <typename T, class Map, class Reduce, bool ACC>
+__device__ __forceinline__ void semiring_ring_body(const CUtensorMap &tmap_a, const CUtensorMap &tmap_b,
+                                                   T *__restrict__ C, unsigned size_n, unsigned size_k,
+                                                   unsigned size_m, unsigned a_step, unsigned b_step) {
   static_assert(sizeof(T) == 4, "ring variant: 4-byte element types");
   using Cfg = SemiringRing;
   constexpr int BM = Cfg::BM, BN = Cfg::BN, BK = Cfg::BK, STAGES = Cfg::STAGES;
@@ -150,18 +150,46 @@ semiring_ring_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_co
         Quad<T> out;
 #pragma unroll
         for (int q = 0; q < 4; ++q) out.v[q] = acc[i][h * 4 + q];
+        if constexpr (ACC) {
+          const Quad<T> old = *reinterpret_cast<const Quad<T> *>(C + row * size_m + col);
+#pragma unroll
+          for (int q = 0; q < 4; ++q) out.v[q] = Reduce::Apply(old.v[q], out.v[q]);
+        }
         *reinterpret_cast<Quad<T> *>(C + row * size_m + col) = out;
       }
     }
   }
 }
 
-// Host side: nullptr A = dry run (load the kernel only).  Returns a cudaError_t value as int.
 template <typename T, class Map, class Reduce>
+__global__ void __launch_bounds__(256, 2)
+semiring_ring_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                     T *__restrict__ C, unsigned size_n, unsigned size_k, unsigned size_m, unsigned a_step,
+                     unsigned b_step) {
+  semiring_ring_body<T, Map, Reduce, false>(tmap_a, tmap_b, C, size_n, size_k, size_m, a_step, b_step);
+}
+
+// C <- Reduce(C_old, A (x) B) (mm_kernel_enqueue_accumulate); instantiated by semiring_accumulate_inst.cu only.
+template <typename T, class Map, class Reduce>
+__global__ void __launch_bounds__(256, 2)
+semiring_accumulate_ring_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                                T *__restrict__ C, unsigned size_n, unsigned size_k, unsigned size_m, unsigned a_step,
+                                unsigned b_step) {
+  semiring_ring_body<T, Map, Reduce, true>(tmap_a, tmap_b, C, size_n, size_k, size_m, a_step, b_step);
+}
+
+// Host side: nullptr A = dry run (load the kernel only).  Returns a cudaError_t value as int.
+template <typename T, class Map, class Reduce, bool ACC>
+constexpr auto semiring_ring_kernel_ptr() {
+  if constexpr (ACC) return semiring_accumulate_ring_kernel<T, Map, Reduce>;
+  else return semiring_ring_kernel<T, Map, Reduce>;
+}
+
+template <typename T, class Map, class Reduce, bool ACC = false>
 int launch_semiring_ring(const void *a, const void *b, void *c, unsigned n, unsigned k, unsigned m, unsigned batch,
                          bool shared_a, bool shared_b, cudaStream_t stream) {
   using Cfg = SemiringRing;
-  auto kernel = semiring_ring_kernel<T, Map, Reduce>;
+  auto kernel = semiring_ring_kernel_ptr<T, Map, Reduce, ACC>();
   cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(Cfg::SMEM_BYTES));
   if (e != cudaSuccess || a == nullptr) return static_cast<int>(e);
   CUtensorMap tmap_a, tmap_b;

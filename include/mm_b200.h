@@ -217,6 +217,35 @@ MM_API int mm_kernel_enqueue_witness(mm_context *ctx, int dtype, int map_op, int
                                      unsigned *w_device, unsigned size_n, unsigned size_k, unsigned size_m,
                                      unsigned batch, void *cuda_stream);
 
+/* ---- accumulation: C <- C (+) (A (x) B) -------------------------------------------------------------
+ * mm_kernel_enqueue_accumulate() takes the arguments of mm_kernel_enqueue_batched() and, for problem p and element
+ * (n, m), writes
+ *     C_new[p,n,m] = R(C_old[p,n,m], P[p,n,m])
+ * where P is the value mm_kernel_enqueue_batched() would store there with the same arguments, flags and tuning (bit
+ * for bit), and R is ONE application of the reduce operator of the path that computed P, in the data type, with
+ * C_old as its FIRST operand:
+ *   Add       C_old + P rounded once to nearest-even (float, double, half, bfloat16); integers wrap modulo 2^32
+ *             (uint8_t modulo 256).  The tensor-core paths are (Multiply, Add): R is this add on the stored P.
+ *   Multiply  C_old * P, likewise
+ *   Min       (C_old < P) ? C_old : P      Max  (P < C_old) ? C_old : P
+ *             For float without MM_FLAG_EXACT: fminf(C_old, P) / fmaxf(C_old, P) (FMNMX), as the plain call.
+ *   And       (C_old != 0 && P != 0) ? 1 : 0
+ * The operand order decides the literal Min / Max at ties of +0 and -0 (Min keeps P, Max keeps P) and with NaN (a
+ * NaN P is kept; a NaN C_old gives P).  Two consequences of defining the result by P:
+ *   - half and bfloat16: P is rounded to 16 bits before the add, so C_new has two roundings (BLAS beta = 1 on a
+ *     wider accumulator has one); the reference's Naive<half> rounds after every operation too;
+ *   - float Add: C_new is not a sequential reduction seeded with C_old: C (+) (A (x) B) means what its parentheses say.
+ * Validation as mm_kernel_enqueue_batched(), in the same order and with the same codes, plus: C (batch*N*M
+ * elements) overlapping A ((shared_a ? 1 : batch)*N*K elements) or B ((shared_b ? 1 : batch)*K*M) by one byte ->
+ * MM_ERR_INVALID.  A and B may overlap each other; adjacent ranges are accepted.  Path selection, scratch
+ * (size it with mm_context_reserve_batched() and the same flags before a stream capture), capture rules,
+ * profiling and mm_kernel_launch_count() are those of the batched call.  Device pointers only.  Callers detect the
+ * feature by this symbol. */
+MM_API int mm_kernel_enqueue_accumulate(mm_context *ctx, int dtype, int map_op, int reduce_op, int flags,
+                                        const void *a_device, const void *b_device, void *c_device,
+                                        unsigned size_n, unsigned size_k, unsigned size_m,
+                                        unsigned batch, void *cuda_stream);
+
 /* Per-phase device timing of enqueued work, for roofline accounting.  With profiling on, every
  * mm_kernel_enqueue()/mm_kernel_execute() records CUDA events on the launching stream around
  * (i) the operand-preparation kernels and (ii) the main compute kernel.  mm_context_profile_read()

@@ -174,6 +174,52 @@ for case in WITNESS:
         ok = ok and np.array_equal(w[i], want)
     print("%-42s %s" % (name, "ok" if ok else "MISMATCH"), flush=True)
     bad += 0 if ok else 1
+# accumulation (mm_kernel_enqueue_accumulate): ragged shapes on every family, one batch with a shared operand; C must
+# equal R(C_old, P) with P the plain batched call (tests/accumulate_naive.py).  These cases have run on an H100 without
+# compute-sanitizer so far.
+import accumulate_naive  # noqa: E402
+
+ACCUMULATE = [
+    ("accumulate wgmma f32", G.FLOAT, G.MULTIPLY, G.ADD, 0, (129, 48, 144), 1),
+    ("accumulate wgmma f32 direct stores", G.FLOAT, G.MULTIPLY, G.ADD, 0, (129, 48, 144), 1, dict(tma_store=0)),
+    ("accumulate wgmma f16 shared B", G.HALF, G.MULTIPLY, G.ADD, G.FLAG_BATCH_SHARED_B, (65, 64, 96), 3),
+    ("accumulate wgmma u8", G.UINT8, G.MULTIPLY, G.ADD, 0, (67, 128, 192), 1),
+    ("accumulate dmma f64 TA", G.DOUBLE, G.MULTIPLY, G.ADD, G.FLAG_TRANSPOSED_A, (66, 16, 72), 1),
+    ("accumulate ring f32 addmin", G.FLOAT, G.ADD, G.MIN, 0, (129, 48, 144), 1),
+    ("accumulate tile bf16 exact", G.BFLOAT16, G.MULTIPLY, G.ADD, G.FLAG_EXACT, (65, 64, 96), 2),
+]
+for case in ACCUMULATE:
+    name, dt, mp, rd, flags, (n, k, m), batch = case[:7]
+    tuning = case[7] if len(case) > 7 else {}
+    if only and only not in name:
+        continue
+    shared_b = bool(flags & G.FLAG_BATCH_SHARED_B)
+    data = [bf16_naive.fill(O, n, k, m, 60 + i) if dt == G.BFLOAT16 else O.fill(dt, n, k, m, 60 + i) for i in range(batch)]
+    ta = bool(flags & G.FLAG_TRANSPOSED_A)
+    a = np.concatenate([(np.ascontiguousarray(d[0].reshape(n, k).T) if ta else d[0]).reshape(-1) for d in data])
+    b = np.concatenate([d[1].reshape(-1) for d in data[:1 if shared_b else batch]])
+    if dt == G.HALF:
+        a = (a.astype(np.float32) * np.float32(0.25)).astype(np.float16)
+    with G.Context(0) as ctx:
+        ctx.set_tuning(**tuning)
+        da, db = ctx.alloc(a.nbytes), ctx.alloc(b.nbytes)
+        dc, dp = (ctx.alloc(batch * n * m * a.itemsize) for _ in range(2))
+        ctx.copy_to_device(da, a)
+        ctx.copy_to_device(db, b)
+        ctx.enqueue_batched(dt, mp, rd, da, db, dp, n, k, m, batch, flags=flags)
+        p = np.empty(batch * n * m, dtype=a.dtype)
+        ctx.copy_to_host(p, dp)
+        c0 = accumulate_naive.c_old(dt, rd, p, 7)
+        ctx.copy_to_device(dc, c0)
+        ctx.enqueue_accumulate(dt, mp, rd, da, db, dc, n, k, m, batch=batch, flags=flags)
+        c = np.empty_like(p)
+        ctx.copy_to_host(c, dc)
+        for x in (da, db, dc, dp):
+            ctx.free(x)
+    fm = dt == G.FLOAT and rd in (G.MIN, G.MAX) and not flags & G.FLAG_EXACT
+    ok = accumulate_naive.same(dt, c, accumulate_naive.reduce_once(dt, rd, c0, p, fm), rd)
+    print("%-42s %s" % (name, "ok" if ok else "MISMATCH"), flush=True)
+    bad += 0 if ok else 1
 # the row-block split on one device listed twice: sliced upload of B, the gather kernel, host barriers
 if not only or "multi" in only:
     for dt, shape in ((G.FLOAT, (300, 128, 272)), (G.HALF, (257, 128, 288)), (G.DOUBLE, (130, 128, 136)),
