@@ -4,11 +4,17 @@
 #include <cuda_runtime.h>
 
 #include <cstdio>
+#include <functional>
 #include <string>
 
 #include "../../include/mm_b200.h"
 
 namespace mm {
+
+// Multi-GPU calls (capi.cu): called by each device's float GEMM path once its rows of A are prepared and before
+// its first GEMM, with its fits word of A (HalfScratch::fits_a, or null without fp16 copies) and the stream that
+// prepared it.  It returns once every device has called it, with the word cleared unless the whole A fits.
+using AgreeFn = std::function<int(unsigned int *fits_a, cudaStream_t stream)>;
 
 // Thread-local error message behind mm_last_error().
 void set_error(const std::string &msg);
@@ -87,6 +93,8 @@ struct GemmArgs {
   bool dry_run = false;
   // mm_kernel_enqueue_accumulate: C <- Reduce(C_old, product), C_old read in the compute kernel's epilogue
   bool accumulate = false;
+  // mm_multi_execute: the devices' agreement on the datapath of the whole A (AgreeFn), or null
+  const AgreeFn *agree = nullptr;
 };
 
 // ---- kernel families (one launcher per translation unit) ---------------------------------------
@@ -98,15 +106,35 @@ int launch_semiring_witness(int dtype, int map_op, int reduce_op, const GemmArgs
 int launch_semiring_accumulate(int dtype, int map_op, int reduce_op, const GemmArgs &args);
 
 // wgmma tensor-core GEMM for (Multiply, Add) float (tf32), half (f16) and uint8_t (u8).
-// The context's scratch holds, in this order: [B operand copy][A operand copy][counters].
+// The context's scratch holds, in this order: [B operand copy][B fp16][A operand copy][A fp16] ... [fits][counters].
 //   B operand copy: the transposed M x K copy wgmma reads K-major, rounded to TF32 for float.
 //   A operand copy: float = A rounded to TF32; any type with MM_FLAG_TRANSPOSED_A = A transposed.
+//   fp16 copies and fits flags (float on the default TF32 datapath only, see HalfScratch): the rounded copies again as
+//   halves, and per distinct operand whether every value of it is exactly a half.
 // A batch keeps one copy per distinct operand (GemmBatch::a_copies / b_copies), packed.
 size_t tcgen05_scratch_bytes(int dtype, unsigned n, unsigned k, unsigned m, int flags, const Tuning &t,
                              const GemmBatch &batch = GemmBatch{});
 size_t tcgen05_bt_bytes(int dtype, unsigned k, unsigned m, int flags, const Tuning &t,
                         unsigned b_copies = 1);  // = offset of the A copy
 int launch_tcgen05(int dtype, const GemmArgs &args, void *scratch, size_t scratch_bytes);
+// Float's fp16 operand copies and their fits flags as the GEMM reads them: a problem whose A and B both fit runs on
+// the f16 wgmma.  All null: TF32 only.
+struct HalfOperands {
+  const void *a = nullptr, *b = nullptr;
+  const unsigned int *fits_a = nullptr, *fits_b = nullptr;
+};
+// Where the preparation writes them.  fits: [one word per B copy][one word per A copy] just before the counters at the
+// scratch's end, set nonzero (cudaMemsetAsync of flag_bytes) before the preparation, cleared by any preparation block
+// that meets a value which is not exactly a normal half or zero (fits_half.h).  All null when the call stays on TF32:
+// not float, MM_FLAG_TF32X3 (its lo parts are far below half range) or the tf32_no_round experiment (raw float bits).
+struct HalfScratch {
+  void *a = nullptr, *b = nullptr;
+  unsigned int *fits_a = nullptr, *fits_b = nullptr;
+  size_t flag_bytes = 0;
+  HalfOperands operands() const { return HalfOperands{a, b, fits_a, fits_b}; }
+};
+HalfScratch tcgen05_half_scratch(void *scratch, size_t scratch_bytes, int dtype, unsigned n, unsigned k, unsigned m,
+                                 int flags, const Tuning &t, const GemmBatch &batch = GemmBatch{});
 // How the kernel consumes B for this configuration.
 bool tcgen05_b_mn(int dtype, int flags, const Tuning &t);      // MN-major (row-major K x M array) vs K-major copy
 bool tcgen05_b_in_place(int dtype, int flags, const Tuning &t);  // no B copy at all (half, MN-major)
@@ -134,9 +162,11 @@ Tcgen05Counters tcgen05_counters(void *scratch, size_t scratch_bytes);
 // a time, in the order the GEMM's rasterisation consumes them) as a co-resident persistent kernel and
 // publishes each panel through ready[panel]; *ready_target receives the count that means "complete".
 // `copies` packed K x M problems of B are prepared into `copies` packed M x K copies (K-major path only).
+// `bt16` / `fits` non-null (HalfScratch): float's K-major copy is also written as halves into `bt16`, and fits[i]
+// cleared when copy i has a value that is not a half.
 int tcgen05_prepare_b(int dtype, const BSource &src, void *bt, unsigned k, unsigned m, int flags, const Tuning &t,
                       const void **b_op, unsigned int *ready, unsigned *ready_target, cudaStream_t stream,
-                      unsigned copies = 1);
+                      unsigned copies = 1, void *bt16 = nullptr, unsigned int *fits = nullptr);
 // Fork / join wrapper around tcgen05_prepare_b for the launchers: decides whether the preparation
 // overlaps the GEMM (float rounding, or any gather of peer slices, with the MN-major B path and a side
 // stream), zeroes the panel counters in stream order, runs the pass on `side` — ENQUEUED BEFORE the
@@ -151,16 +181,18 @@ struct PreparedB {
 };
 int tcgen05_prepare_b_async(int dtype, const BSource &src, void *local_b, void *scratch, size_t scratch_bytes,
                             unsigned k, unsigned m, int flags, const Tuning &t, cudaStream_t stream, cudaStream_t side,
-                            cudaEvent_t ev_fork, cudaEvent_t ev_join, PreparedB *out, unsigned copies = 1);
-// `copies` packed problems of `rows` rows each.
+                            cudaEvent_t ev_fork, cudaEvent_t ev_join, PreparedB *out, unsigned copies = 1,
+                            void *bt16 = nullptr, unsigned int *fits = nullptr);
+// `copies` packed problems of `rows` rows each.  `aprep16` / `fits` as for tcgen05_prepare_b: problem i clears fits[i].
 int tcgen05_prepare_a(int dtype, const void *a, void *aprep, unsigned rows, unsigned k, int flags, const Tuning &t,
-                      const void **a_op, cudaStream_t stream, unsigned copies = 1);
+                      const void **a_op, cudaStream_t stream, unsigned copies = 1, void *aprep16 = nullptr,
+                      unsigned int *fits = nullptr);
 // `tile_sync`: device counter for the kernel's soft wave barrier, or null.  `b_ready` non-null: the
 // producer waits for b_ready[column tile] >= b_ready_target before it fetches a tile's B panel.
 int tcgen05_gemm(int dtype, const void *a_op, const void *b_op, void *c, unsigned rows, unsigned k, unsigned m,
                  int flags, const Tuning &t, unsigned int *tile_sync, const unsigned int *b_ready,
                  unsigned b_ready_target, cudaStream_t stream, const GemmBatch &batch = GemmBatch{},
-                 bool accumulate = false);
+                 bool accumulate = false, const HalfOperands &half = HalfOperands{});
 constexpr size_t kTcgen05TailBytes = 256 + 64 * 1024;  // [panel counters, 64 KiB][wave-barrier counter, 256 B]
 // Generic gather of row-sliced B into one local array (identity transform): what the multi-GPU path
 // uses for the kernel families that read B as is (double, semirings, half).

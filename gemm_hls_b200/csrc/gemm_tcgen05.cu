@@ -28,6 +28,10 @@
 //     A and B are therefore rounded to nearest TF32 (cvt.rna.tf32.f32) into scratch copies first.
 //   * half, bfloat16 and uint8_t A are K-major as stored; B is transposed.  bfloat16 moves the same bits as
 //     half, so it shares half's transpose kernel.
+//   * A value rounded to TF32 keeps 10 mantissa bits, as many as a half has.  So the same passes also write the
+//     rounded operands as halves and note, per distinct operand, whether every value is 0 or a normal half
+//     (fits_half.h).  A problem whose A and B both fit runs on the f16 wgmma, which multiplies the very same values
+//     at twice the TF32 issue rate (gemm_wgmma.cuh); any other problem stays on TF32.
 //
 // The GEMM kernel and its launcher are in gemm_wgmma.cuh.  This unit instantiates them for tf32, f16 and
 // u8; the bf16 instantiations are in gemm_wgmma_bf16.cu, the accumulate kernels in gemm_wgmma_acc.cu.
@@ -41,6 +45,7 @@
 #include <vector>
 
 #include "common.cuh"
+#include "fits_half.h"
 #include "gemm_wgmma.cuh"
 #include "ptx_sm90.cuh"
 #include "tma_host.cuh"
@@ -60,10 +65,21 @@ __device__ __forceinline__ float round_tf32(float x) {
 
 // ---- operand preparation ------------------------------------------------------------------------
 
-// dst[i] = rna_tf32(src[i]); count is a multiple of 4 (K % 16 == 0).
+__device__ __forceinline__ uint32_t half2_bits(float lo, float hi) {
+  const __half2 h = __floats2half2_rn(lo, hi);
+  return *reinterpret_cast<const uint32_t *>(&h);
+}
+
+// dst[i] = rna_tf32(src[i]); count4 float4 per problem, blockIdx.y = problem of a batch (packed).  HALF: dst16 gets the
+// same values as halves, and fits[problem] is cleared when one of them is not exactly a half (one store per block).
+template <bool HALF>
 __global__ void __launch_bounds__(256)
-round_tf32_kernel(const float4 *__restrict__ src, float4 *__restrict__ dst, size_t count4) {
+round_tf32_kernel(const float4 *__restrict__ src, float4 *__restrict__ dst, size_t count4, uint2 *__restrict__ dst16,
+                  unsigned int *__restrict__ fits) {
+  src += size_t(blockIdx.y) * count4;
+  dst += size_t(blockIdx.y) * count4;
   const size_t stride = size_t(gridDim.x) * blockDim.x;
+  bool fit = true;
   for (size_t i = size_t(blockIdx.x) * blockDim.x + threadIdx.x; i < count4; i += stride) {
     float4 v = src[i];
     v.x = round_tf32(v.x);
@@ -71,6 +87,14 @@ round_tf32_kernel(const float4 *__restrict__ src, float4 *__restrict__ dst, size
     v.z = round_tf32(v.z);
     v.w = round_tf32(v.w);
     dst[i] = v;
+    if constexpr (HALF) {
+      dst16[size_t(blockIdx.y) * count4 + i] = make_uint2(half2_bits(v.x, v.y), half2_bits(v.z, v.w));
+      fit = fit && tf32_fits_half(__float_as_uint(v.x)) && tf32_fits_half(__float_as_uint(v.y)) &&
+            tf32_fits_half(__float_as_uint(v.z)) && tf32_fits_half(__float_as_uint(v.w));
+    }
+  }
+  if constexpr (HALF) {
+    if (__syncthreads_or(!fit) && threadIdx.x == 0) fits[blockIdx.y] = 0u;
   }
 }
 
@@ -156,11 +180,12 @@ __device__ __forceinline__ float prep_value<float, true>(float x) {
 
 // dst[c][r] = f(src[r][c]) for src of shape src_rows x src_cols (row-major): 64 x 64 tiles through
 // shared memory so that both the reads and the writes are row-contiguous.  blockIdx.z = problem of a
-// batch: packed sources, packed destinations.
+// batch: packed sources, packed destinations.  ROUND (float to TF32): dst16 gets the rounded values as halves too, and
+// fits[problem] is cleared when one of them is not exactly a half, as in round_tf32_kernel.
 template <typename T, bool ROUND>
 __global__ void __launch_bounds__(256)
 transpose_prep_kernel(const T *__restrict__ src, T *__restrict__ dst, uint32_t src_rows,
-                      uint32_t src_cols) {
+                      uint32_t src_cols, __half *__restrict__ dst16, unsigned int *__restrict__ fits) {
   constexpr int TILE = 64;
   constexpr int PAD = (sizeof(T) >= 4) ? 1 : 2;
   __shared__ T tile[TILE][TILE + PAD];
@@ -176,10 +201,21 @@ transpose_prep_kernel(const T *__restrict__ src, T *__restrict__ dst, uint32_t s
     if (r < src_rows && c < src_cols) tile[i][x] = prep_value<T, ROUND>(src[size_t(r) * src_cols + c]);
   }
   __syncthreads();
+  bool fit = true;
 #pragma unroll 4
   for (int i = y; i < TILE; i += 4) {
     const uint32_t c = c0 + i, r = r0 + x;  // dst row = src col
-    if (c < src_cols && r < src_rows) dst[size_t(c) * src_rows + r] = tile[x][i];
+    if (c < src_cols && r < src_rows) {
+      const T v = tile[x][i];
+      dst[size_t(c) * src_rows + r] = v;
+      if constexpr (ROUND) {
+        dst16[size_t(blockIdx.z) * src_rows * src_cols + size_t(c) * src_rows + r] = __float2half_rn(v);
+        fit = fit && tf32_fits_half(__float_as_uint(v));
+      }
+    }
+  }
+  if constexpr (ROUND) {
+    if (__syncthreads_or(!fit) && threadIdx.x == 0) fits[blockIdx.z] = 0u;
   }
 }
 
@@ -268,10 +304,30 @@ size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
 template <typename T, bool ROUND>
 void launch_transpose(const void *src, void *dst, uint32_t src_rows, uint32_t src_cols, cudaStream_t stream,
-                      unsigned copies) {
+                      unsigned copies, void *dst16 = nullptr, unsigned int *fits = nullptr) {
   dim3 grid((src_cols + 63) / 64, (src_rows + 63) / 64, copies);
   transpose_prep_kernel<T, ROUND><<<grid, 256, 0, stream>>>(static_cast<const T *>(src), static_cast<T *>(dst),
-                                                           src_rows, src_cols);
+                                                           src_rows, src_cols, static_cast<__half *>(dst16), fits);
+}
+
+// Rounds `copies` packed problems of count4 float4 each; with `dst16` the fp16 copies and fits flags too.
+int launch_round(const void *src, void *dst, size_t count4, unsigned copies, void *dst16, unsigned int *fits,
+                 cudaStream_t stream) {
+  const int blocks = int(std::min<size_t>((count4 + 255) / 256, size_t(num_sms()) * 16));
+  const dim3 grid(std::max(blocks, 1), copies);
+  const float4 *s = static_cast<const float4 *>(src);
+  float4 *d = static_cast<float4 *>(dst);
+  if (dst16 != nullptr) {
+    // see tcgen05_prepare_b
+    MM_CUDA_TRY(cudaFuncSetAttribute(round_tf32_kernel<true>, cudaFuncAttributePreferredSharedMemoryCarveout,
+                                     cudaSharedmemCarveoutMaxShared));
+    round_tf32_kernel<true><<<grid, 256, 0, stream>>>(s, d, count4, static_cast<uint2 *>(dst16), fits);
+  } else {
+    MM_CUDA_TRY(cudaFuncSetAttribute(round_tf32_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout,
+                                     cudaSharedmemCarveoutMaxShared));
+    round_tf32_kernel<false><<<grid, 256, 0, stream>>>(s, d, count4, nullptr, nullptr);
+  }
+  return MM_OK;
 }
 
 bool split3(int dtype, int flags) { return dtype == MM_DTYPE_FLOAT && (flags & MM_FLAG_TF32X3); }
@@ -314,20 +370,48 @@ bool tcgen05_b_in_place(int dtype, int flags, const Tuning &t) {
   return tcgen05_b_mn(dtype, flags, t) && (dtype == MM_DTYPE_HALF || dtype == MM_DTYPE_UINT8 || t.tf32_no_round());
 }
 
+// float on the default TF32 datapath: the preparation also writes fp16 copies and fits flags (HalfScratch)
+bool half_copies(int dtype, int flags, const Tuning &t) {
+  return dtype == MM_DTYPE_FLOAT && !split3(dtype, flags) && !t.tf32_no_round();
+}
+
+size_t b_copy_bytes(int dtype, unsigned k, unsigned m, int flags, unsigned b_copies) {
+  return align_up(size_t(b_copies) * m * k * elem_bytes(dtype) * (split3(dtype, flags) ? 3 : 1), 1024);
+}
+size_t a_copy_bytes(int dtype, unsigned n, unsigned k, int flags, unsigned a_copies) {
+  if (dtype != MM_DTYPE_FLOAT && !(flags & MM_FLAG_TRANSPOSED_A)) return 0;
+  return align_up(size_t(a_copies) * n * k * elem_bytes(dtype) * (split3(dtype, flags) ? 3 : 1), 1024);
+}
+size_t fits_bytes(const GemmBatch &batch) {
+  return align_up(size_t(batch.a_copies() + batch.b_copies()) * sizeof(unsigned int), 1024);
+}
+
 size_t tcgen05_bt_bytes(int dtype, unsigned k, unsigned m, int flags, const Tuning &t, unsigned b_copies) {
   if (tcgen05_b_in_place(dtype, flags, t)) return 0;
-  const size_t eb = elem_bytes(dtype);
-  return align_up(size_t(b_copies) * m * k * eb * (split3(dtype, flags) ? 3 : 1), 1024);
+  const size_t fp16 = half_copies(dtype, flags, t) ? align_up(size_t(b_copies) * m * k * 2, 1024) : 0;
+  return b_copy_bytes(dtype, k, m, flags, b_copies) + fp16;  // [B copy][B fp16]
 }
 
 size_t tcgen05_scratch_bytes(int dtype, unsigned n, unsigned k, unsigned m, int flags, const Tuning &t,
                              const GemmBatch &batch) {
-  const size_t eb = elem_bytes(dtype);
   size_t bytes = TAIL_BYTES + tcgen05_bt_bytes(dtype, k, m, flags, t, batch.b_copies());  // counters (tail) + B copies
-  if (dtype == MM_DTYPE_FLOAT || (flags & MM_FLAG_TRANSPOSED_A)) {
-    bytes += align_up(size_t(batch.a_copies()) * n * k * eb * (split3(dtype, flags) ? 3 : 1), 1024);
-  }
+  bytes += a_copy_bytes(dtype, n, k, flags, batch.a_copies());
+  if (half_copies(dtype, flags, t)) bytes += align_up(size_t(batch.a_copies()) * n * k * 2, 1024) + fits_bytes(batch);
   return bytes;
+}
+
+HalfScratch tcgen05_half_scratch(void *scratch, size_t scratch_bytes, int dtype, unsigned n, unsigned k, unsigned m,
+                                 int flags, const Tuning &t, const GemmBatch &batch) {
+  HalfScratch h;
+  if (!half_copies(dtype, flags, t)) return h;
+  unsigned char *sp = static_cast<unsigned char *>(scratch);
+  const size_t bt = tcgen05_bt_bytes(dtype, k, m, flags, t, batch.b_copies());
+  h.b = sp + b_copy_bytes(dtype, k, m, flags, batch.b_copies());
+  h.a = sp + bt + a_copy_bytes(dtype, n, k, flags, batch.a_copies());
+  h.flag_bytes = fits_bytes(batch);
+  h.fits_b = reinterpret_cast<unsigned int *>(sp + scratch_bytes - TAIL_BYTES - h.flag_bytes);
+  h.fits_a = h.fits_b + batch.b_copies();
+  return h;
 }
 
 // Copy row-sliced B (slices on peer GPUs) into one local array: the NVLink all-gather of the
@@ -339,7 +423,7 @@ int gather_b_rows(const BSource &src, void *dst, size_t elem_bytes, unsigned k, 
 
 int tcgen05_prepare_b(int dtype, const BSource &src, void *bt, unsigned k, unsigned m, int flags, const Tuning &t,
                       const void **b_op, unsigned int *ready, unsigned *ready_target, cudaStream_t stream,
-                      unsigned copies) {
+                      unsigned copies, void *bt16, unsigned int *fits) {
   *b_op = bt;
   if (ready_target) *ready_target = 0;
   const bool parts = src.src != nullptr;
@@ -355,11 +439,8 @@ int tcgen05_prepare_b(int dtype, const BSource &src, void *bt, unsigned k, unsig
     if (!in_place && !parts && ready == nullptr) {
       // one local array, nobody waiting on panels: the flat elementwise pass (6.3 TB/s against the panel
       // kernel's 5.1 on a 512 MiB block — the panel order costs row-segment locality)
-      MM_CUDA_TRY(cudaFuncSetAttribute(round_tf32_kernel, cudaFuncAttributePreferredSharedMemoryCarveout,
-                                       cudaSharedmemCarveoutMaxShared));
-      const size_t count4 = size_t(k) * m / 4;
-      const int blocks = int(std::min<size_t>((count4 + 255) / 256, size_t(num_sms()) * 16));
-      round_tf32_kernel<<<blocks, 256, 0, stream>>>(static_cast<const float4 *>(src.b), static_cast<float4 *>(bt), count4);
+      const int rc = launch_round(src.b, bt, size_t(k) * m / 4, 1, nullptr, nullptr, stream);
+      if (rc != MM_OK) return rc;
       MM_CUDA_TRY(cudaGetLastError());
       return MM_OK;
     }
@@ -392,7 +473,7 @@ int tcgen05_prepare_b(int dtype, const BSource &src, void *bt, unsigned k, unsig
     if (t.tf32_no_round()) {
       launch_transpose<float, false>(b, bt, k, m, stream, copies);
     } else {
-      launch_transpose<float, true>(b, bt, k, m, stream, copies);
+      launch_transpose<float, true>(b, bt, k, m, stream, copies, bt16, fits);
     }
   } else if (dtype == MM_DTYPE_UINT8) {
     launch_transpose<unsigned char, false>(b, bt, k, m, stream, copies);
@@ -408,7 +489,7 @@ int tcgen05_prepare_b(int dtype, const BSource &src, void *bt, unsigned k, unsig
 // matrices) is transposed into `aprep`.  *a_op receives the operand pointer.  `copies` packed problems:
 // the row-wise passes run over copies * rows rows, the transposes take the problem from blockIdx.z.
 int tcgen05_prepare_a(int dtype, const void *a, void *aprep, unsigned rows, unsigned k, int flags, const Tuning &t,
-                      const void **a_op, cudaStream_t stream, unsigned copies) {
+                      const void **a_op, cudaStream_t stream, unsigned copies, void *aprep16, unsigned int *fits) {
   const bool transposed = (flags & MM_FLAG_TRANSPOSED_A) != 0;
   const size_t all_rows = size_t(copies) * rows;
   *a_op = a;
@@ -429,16 +510,12 @@ int tcgen05_prepare_a(int dtype, const void *a, void *aprep, unsigned rows, unsi
       if (t.tf32_no_round()) {
         launch_transpose<float, false>(a, aprep, k, rows, stream, copies);
       } else {
-        launch_transpose<float, true>(a, aprep, k, rows, stream, copies);  // A stored K x N -> N x K
+        launch_transpose<float, true>(a, aprep, k, rows, stream, copies, aprep16, fits);  // A stored K x N -> N x K
       }
       *a_op = aprep;
     } else if (!t.tf32_no_round()) {
-      MM_CUDA_TRY(cudaFuncSetAttribute(round_tf32_kernel, cudaFuncAttributePreferredSharedMemoryCarveout,
-                                       cudaSharedmemCarveoutMaxShared));  // see tcgen05_prepare_b
-      const size_t count4 = all_rows * k / 4;
-      const int blocks = int(std::min<size_t>((count4 + 255) / 256, size_t(num_sms()) * 16));
-      round_tf32_kernel<<<blocks, 256, 0, stream>>>(static_cast<const float4 *>(a),
-                                                   static_cast<float4 *>(aprep), count4);
+      const int rc = launch_round(a, aprep, size_t(rows) * k / 4, copies, aprep16, fits, stream);
+      if (rc != MM_OK) return rc;
       *a_op = aprep;
     }
   } else if (transposed) {
@@ -454,21 +531,21 @@ namespace {
 int gemm_dispatch(int dtype, const void *a_op, const void *b_op, void *c, unsigned rows, unsigned k, unsigned m,
                   int flags, const Tuning &t, unsigned int *tile_sync, const unsigned int *b_ready,
                   unsigned b_ready_target, bool attributes_only, cudaStream_t stream, const GemmBatch &batch,
-                  bool accumulate = false) {
+                  bool accumulate = false, const HalfOperands &half = HalfOperands{}) {
   if (accumulate) {
     if (split3(dtype, flags)) k *= 3;
     return wgmma_accumulate_gemm(dtype, a_op, b_op, c, rows, k, m, t, tile_sync, b_ready, b_ready_target,
-                                 attributes_only, stream, batch);
+                                 attributes_only, stream, batch, half);
   }
   if (dtype == MM_DTYPE_BFLOAT16) {
     return wgmma_bf16_gemm(a_op, b_op, c, rows, k, m, t, tile_sync, b_ready, b_ready_target, attributes_only, stream,
                            batch);
   }
   if (split3(dtype, flags)) k *= 3;  // the operands carry [hi|hi|lo] x [hi|lo|hi] per 16-block of K
-  CUtensorMap maps[3];
+  CUtensorMap maps[5];
   LaunchPlan plan;
   const int rc = plan_gemm(dtype, a_op, b_op, c, rows, k, m, t, tile_sync, b_ready, b_ready_target, attributes_only,
-                           stream, batch, maps, &plan);
+                           stream, batch, half, maps, &plan);
   if (rc != MM_OK) return rc;
   const int cg = t.cta_group(), bn = t.block_n();
   if (dtype == MM_DTYPE_UINT8) return dispatch_variant<ptx::KIND_I8, unsigned char>(cg, bn, plan);
@@ -479,23 +556,26 @@ int gemm_dispatch(int dtype, const void *a_op, const void *b_op, void *c, unsign
 }  // namespace
 
 // C[rows x m] = Aop[rows x k] * B on the tensor cores; `b_op` as returned by tcgen05_prepare_b.  `accumulate`:
-// C <- C + that product, by the accumulate kernels.
+// C <- C + that product, by the accumulate kernels.  `half`: float's fp16 copies and fits flags, or empty.
 int tcgen05_gemm(int dtype, const void *a_op, const void *b_op, void *c, unsigned rows, unsigned k, unsigned m,
                  int flags, const Tuning &t, unsigned int *tile_sync, const unsigned int *b_ready,
-                 unsigned b_ready_target, cudaStream_t stream, const GemmBatch &batch, bool accumulate) {
+                 unsigned b_ready_target, cudaStream_t stream, const GemmBatch &batch, bool accumulate,
+                 const HalfOperands &half) {
   return gemm_dispatch(dtype, a_op, b_op, c, rows, k, m, flags, t, tile_sync, b_ready, b_ready_target, false, stream,
-                       batch, accumulate);
+                       batch, accumulate, half);
 }
 
 int tcgen05_prepare_b_async(int dtype, const BSource &src, void *local_b, void *scratch, size_t scratch_bytes,
                             unsigned k, unsigned m, int flags, const Tuning &t, cudaStream_t stream, cudaStream_t side,
-                            cudaEvent_t ev_fork, cudaEvent_t ev_join, PreparedB *out, unsigned copies) {
+                            cudaEvent_t ev_fork, cudaEvent_t ev_join, PreparedB *out, unsigned copies, void *bt16,
+                            unsigned int *fits) {
   *out = PreparedB{};
   const bool in_place = tcgen05_b_in_place(dtype, flags, t);
   const bool parts = src.src != nullptr;
   if (copies != 1) {
     if (parts) return fail(MM_ERR_UNSUPPORTED, "batched calls take B from one array");
-    return tcgen05_prepare_b(dtype, src, scratch, k, m, flags, t, &out->b_op, nullptr, nullptr, stream, copies);
+    return tcgen05_prepare_b(dtype, src, scratch, k, m, flags, t, &out->b_op, nullptr, nullptr, stream, copies, bt16,
+                             fits);
   }
   if (parts && !tcgen05_b_mn(dtype, flags, t)) {
     // K-major copy requested (tuning / 3xTF32): assemble the slices first, then transpose locally
@@ -503,7 +583,7 @@ int tcgen05_prepare_b_async(int dtype, const BSource &src, void *local_b, void *
     if (rc != MM_OK) return rc;
     BSource whole;
     whole.b = local_b;
-    return tcgen05_prepare_b(dtype, whole, scratch, k, m, flags, t, &out->b_op, nullptr, nullptr, stream);
+    return tcgen05_prepare_b(dtype, whole, scratch, k, m, flags, t, &out->b_op, nullptr, nullptr, stream, 1, bt16, fits);
   }
   void *bt = in_place ? local_b : scratch;
   const Tcgen05Counters cnt = tcgen05_counters(scratch, scratch_bytes);
@@ -511,7 +591,7 @@ int tcgen05_prepare_b_async(int dtype, const BSource &src, void *local_b, void *
   // the panel kernel runs (float rounding, or a gather of slices), a second stream exists, the tuning allows it
   const bool overlap = side != nullptr && t.b_overlap() != 0 && tcgen05_b_mn(dtype, flags, t) && (!in_place || parts) &&
                        panels <= B_READY_BYTES / sizeof(unsigned int);
-  if (!overlap) return tcgen05_prepare_b(dtype, src, bt, k, m, flags, t, &out->b_op, nullptr, nullptr, stream);
+  if (!overlap) return tcgen05_prepare_b(dtype, src, bt, k, m, flags, t, &out->b_op, nullptr, nullptr, stream, 1, bt16, fits);
   MM_CUDA_TRY(cudaMemsetAsync(cnt.b_ready, 0, panels * sizeof(unsigned int), stream));
   MM_CUDA_TRY(cudaEventRecord(ev_fork, stream));
   MM_CUDA_TRY(cudaStreamWaitEvent(side, ev_fork, 0));
@@ -531,7 +611,8 @@ int launch_tcgen05(int dtype, const GemmArgs &g, void *scratch, size_t scratch_b
   if (g.dry_run) {
     // force the lazily loaded kernels in (prep + the GEMM variant this tuning selects) and the driver entry point
     cudaFuncAttributes attr;
-    MM_CUDA_TRY(cudaFuncGetAttributes(&attr, round_tf32_kernel));
+    MM_CUDA_TRY(cudaFuncGetAttributes(&attr, round_tf32_kernel<true>));
+    MM_CUDA_TRY(cudaFuncGetAttributes(&attr, round_tf32_kernel<false>));
     MM_CUDA_TRY(cudaFuncGetAttributes(&attr, prep_b_panels_kernel<true>));
     MM_CUDA_TRY(cudaFuncGetAttributes(&attr, prep_b_panels_kernel<false>));
     MM_CUDA_TRY(cudaFuncGetAttributes(&attr, transpose_prep_kernel<float, true>));
@@ -539,7 +620,7 @@ int launch_tcgen05(int dtype, const GemmArgs &g, void *scratch, size_t scratch_b
     MM_CUDA_TRY(cudaFuncGetAttributes(&attr, transpose_prep_kernel<unsigned char, false>));
     if (!get_encode_fn()) return fail(MM_ERR_CUDA, "cuTensorMapEncodeTiled entry point not available");
     return gemm_dispatch(dtype, nullptr, nullptr, nullptr, g.n, g.k, g.m, g.flags, t, nullptr, nullptr, 0, true, g.stream,
-                         g.batch);
+                         g.batch, g.accumulate);
   }
   if (scratch_bytes < tcgen05_scratch_bytes(dtype, g.n, g.k, g.m, g.flags, t, g.batch)) {
     return fail(MM_ERR_INVALID, "tcgen05 scratch too small");
@@ -551,14 +632,20 @@ int launch_tcgen05(int dtype, const GemmArgs &g, void *scratch, size_t scratch_b
   src.b = g.b;
   PreparedB pb;
   const void *a_op = nullptr;
+  const HalfScratch hs = tcgen05_half_scratch(scratch, scratch_bytes, dtype, g.n, g.k, g.m, g.flags, t, g.batch);
+  if (hs.fits_b) MM_CUDA_TRY(cudaMemsetAsync(hs.fits_b, 1, hs.flag_bytes, g.stream));  // every operand fits until seen
   // one preparation pass per operand for the whole batch; a shared operand is prepared once
   int rc = tcgen05_prepare_b_async(dtype, src, nullptr, scratch, scratch_bytes, g.k, g.m, g.flags, t, g.stream,
-                                   g.side_stream, g.ev_fork, g.ev_join, &pb, g.batch.b_copies());
-  if (rc == MM_OK) rc = tcgen05_prepare_a(dtype, g.a, aprep, g.n, g.k, g.flags, t, &a_op, g.stream, g.batch.a_copies());
+                                   g.side_stream, g.ev_fork, g.ev_join, &pb, g.batch.b_copies(), hs.b, hs.fits_b);
+  if (rc == MM_OK) {
+    rc = tcgen05_prepare_a(dtype, g.a, aprep, g.n, g.k, g.flags, t, &a_op, g.stream, g.batch.a_copies(), hs.a,
+                           hs.fits_a);
+  }
+  if (rc == MM_OK && g.agree != nullptr) rc = (*g.agree)(hs.fits_a, g.stream);
   if (rc == MM_OK && g.ev_prep_done) cudaEventRecord(g.ev_prep_done, g.stream);
   if (rc == MM_OK) {
     rc = tcgen05_gemm(dtype, a_op, pb.b_op, g.c, g.n, g.k, g.m, g.flags, t, cnt.tile_sync, pb.ready, pb.ready_target,
-                      g.stream, g.batch, g.accumulate);
+                      g.stream, g.batch, g.accumulate, hs.operands());
   }
   if (pb.forked) cudaStreamWaitEvent(g.stream, g.ev_join, 0);  // join, on the error paths too
   return rc;

@@ -12,6 +12,7 @@
 
 #include <algorithm>
 #include <cstring>
+#include <type_traits>
 
 #include "common.cuh"
 #include "ptx_sm90.cuh"
@@ -180,13 +181,20 @@ struct GemmParams {
   uint64_t l2_policy;
   unsigned int *tile_sync;        // soft wave-barrier counter or null
   const unsigned int *b_ready;    // per column tile: preparation items finished, or null (B complete)
+  // float only: per distinct A (B) operand of the batch, nonzero when every TF32-rounded value of it is exactly a half
+  // (gemm_tcgen05.cu); a tile whose A and B both fit reads the fp16 copies and runs on the f16 wgmma.  Null: TF32 only.
+  const unsigned int *fits_a, *fits_b;
 };
 
 // C[rows x cols] = A'[rows x k] * B'^T ; A' (rows x k) and B' (cols x k) K-major.  CG == 2 must be
 // launched with cluster dimension (2, 1, 1).  ACC: C = C_old + A'B'^T, the add applied to the rounded product in
 // the epilogue (gemm_wgmma_accumulate_kernel); nothing else differs.
+// KIND_TF32 has two datapaths, chosen per tile from the problem's fits flags (GemmParams::fits_a / fits_b): the TF32
+// operands through tmap_a / tmap_b and wgmma tf32, or their fp16 copies (the same values, exactly) through tmap_a16 /
+// tmap_b16 and wgmma f16 at twice the issue rate.  A stage is 128 bytes of K either way: 32 floats or 64 halves.
 template <int KIND, typename TOut, int CG, int BN, bool ACC>
 __device__ __forceinline__ void gemm_wgmma_body(const CUtensorMap &tmap_a, const CUtensorMap &tmap_b,
+                                                const CUtensorMap &tmap_a16, const CUtensorMap &tmap_b16,
                                                 const CUtensorMap &tmap_c, TOut *__restrict__ C, const GemmParams &p) {
   using G = Geo<CG, BN>;
   constexpr int ELEM_BYTES = (KIND == ptx::KIND_TF32) ? 4 : (KIND == ptx::KIND_I8 ? 1 : 2);  // f16, bf16: 2
@@ -213,11 +221,22 @@ __device__ __forceinline__ void gemm_wgmma_body(const CUtensorMap &tmap_a, const
   const uint32_t tiles_c = (cols + BN - 1) / BN;
   const uint32_t num_tiles = p.batch * tiles_r * tiles_c;
   const uint32_t num_kb = (p.k_bytes + BLOCK_K_BYTES - 1) / BLOCK_K_BYTES;
+  const uint32_t num_kb16 = (p.k_bytes / 2 + BLOCK_K_BYTES - 1) / BLOCK_K_BYTES;  // the fp16 copies: half the bytes
+  // both roles of the CTA take the same datapath for a tile: the producer loads what the consumers multiply
+  auto half_tile = [&](const TileCoord &tc) -> bool {
+    if constexpr (KIND != ptx::KIND_TF32) return false;
+    if (p.fits_a == nullptr) return false;
+    return p.fits_a[p.a_prob_rows ? tc.prob : 0u] != 0u && p.fits_b[p.b_prob_rows ? tc.prob : 0u] != 0u;
+  };
 
   if (threadIdx.x == 0) {
     ptx::prefetch_tensormap(&tmap_a);
     ptx::prefetch_tensormap(&tmap_b);
     if (p.tma_store) ptx::prefetch_tensormap(&tmap_c);
+    if (KIND == ptx::KIND_TF32 && p.fits_a != nullptr) {
+      ptx::prefetch_tensormap(&tmap_a16);
+      ptx::prefetch_tensormap(&tmap_b16);
+    }
     for (int s = 0; s < STAGES; ++s) {
       // full: the own producer's arrive.expect_tx (bytes of A, both halves of B -- the peer's half
       // arrives by its multicast).  empty: one arrival per consumer warp of EVERY CTA of the cluster,
@@ -263,17 +282,22 @@ __device__ __forceinline__ void gemm_wgmma_body(const CUtensorMap &tmap_a, const
           asm volatile("fence.proxy.async.global;" ::: "memory");  // generic-proxy writes -> TMA reads
           ready_panel = int32_t(tc.c);
         }
-        for (uint32_t kb = 0; kb < num_kb; ++kb) {
+        const bool h = half_tile(tc);
+        const CUtensorMap *map_a = h ? &tmap_a16 : &tmap_a;
+        const CUtensorMap *map_b = h ? &tmap_b16 : &tmap_b;
+        const uint32_t tile_kb = h ? num_kb16 : num_kb;
+        const int32_t kb_elems = h ? BLOCK_K_BYTES / 2 : BLOCK_K_ELEMS;
+        for (uint32_t kb = 0; kb < tile_kb; ++kb) {
           ptx::mbar_wait(empty_bar(stage), phase ^ 1);
           const uint32_t sa = smem_a0 + stage * G::A_STAGE_BYTES;
           const uint32_t sb = smem_b0 + stage * G::B_STAGE_BYTES + cta_rank * G::LOAD_N * BLOCK_K_BYTES;
-          const int32_t k0 = kb * BLOCK_K_ELEMS;
+          const int32_t k0 = kb * kb_elems;
           ptx::mbar_arrive_expect_tx(full_bar(stage), G::STAGE_BYTES);
-          ptx::tma_load_2d(sa, &tmap_a, full_bar(stage), k0, a_row, p.l2_policy);
+          ptx::tma_load_2d(sa, map_a, full_bar(stage), k0, a_row, p.l2_policy);
           if (CG == 1) {
-            ptx::tma_load_2d(sb, &tmap_b, full_bar(stage), k0, b_row, p.l2_policy);
+            ptx::tma_load_2d(sb, map_b, full_bar(stage), k0, b_row, p.l2_policy);
           } else {
-            ptx::tma_load_2d_multicast(sb, &tmap_b, full_bar(stage), k0, b_row, 0x3, p.l2_policy);
+            ptx::tma_load_2d_multicast(sb, map_b, full_bar(stage), k0, b_row, 0x3, p.l2_policy);
           }
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
@@ -291,31 +315,41 @@ __device__ __forceinline__ void gemm_wgmma_body(const CUtensorMap &tmap_a, const
     uint32_t acc[BN / 2];
     for (uint32_t t = group_id; t < num_tiles; t += num_groups) {
       const TileCoord tc = tile_coord(t, tiles_r, tiles_c, p.raster_group);
-      uint32_t prev = 0;
-      for (uint32_t kb = 0; kb < num_kb; ++kb) {
-        ptx::mbar_wait(full_bar(stage), phase);
-        const uint64_t adesc = ptx::make_smem_desc_k_sw128(smem_a0 + stage * G::A_STAGE_BYTES + wg * 64 * BLOCK_K_BYTES);
-        const uint64_t bdesc = ptx::make_smem_desc_k_sw128(smem_b0 + stage * G::B_STAGE_BYTES);
-        ptx::wgmma_fence();
+      // The k-loop once per datapath, each a whole wgmma pipeline up to its final wait: a branch between the issue
+      // and the wait of one pipeline would make ptxas serialise every wgmma.
+      auto mainloop = [&](auto kind, uint32_t tile_kb) {
+        uint32_t prev = 0;
+        for (uint32_t kb = 0; kb < tile_kb; ++kb) {
+          ptx::mbar_wait(full_bar(stage), phase);
+          const uint64_t adesc = ptx::make_smem_desc_k_sw128(smem_a0 + stage * G::A_STAGE_BYTES + wg * 64 * BLOCK_K_BYTES);
+          const uint64_t bdesc = ptx::make_smem_desc_k_sw128(smem_b0 + stage * G::B_STAGE_BYTES);
+          ptx::wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < BLOCK_K_BYTES / WGMMA_K_BYTES; ++k) {
-          ptx::wgmma<KIND, BN>(acc, adesc + uint64_t(k * (WGMMA_K_BYTES >> 4)), bdesc + uint64_t(k * (WGMMA_K_BYTES >> 4)),
-                               (kb | uint32_t(k)) != 0u ? 1u : 0u);
+          for (int k = 0; k < BLOCK_K_BYTES / WGMMA_K_BYTES; ++k) {
+            ptx::wgmma<decltype(kind)::value, BN>(acc, adesc + uint64_t(k * (WGMMA_K_BYTES >> 4)),
+                                                  bdesc + uint64_t(k * (WGMMA_K_BYTES >> 4)),
+                                                  (kb | uint32_t(k)) != 0u ? 1u : 0u);
+          }
+          ptx::wgmma_commit();
+          // keep one group in flight: the previous k-block's group has retired, its stage is free
+          ptx::wgmma_wait<1>();
+          if (kb > 0 && lane == 0) {
+            ptx::mbar_arrive(empty_bar(prev));
+            if (CG == 2) ptx::mbar_arrive_cluster(empty_bar(prev), peer);
+          }
+          prev = stage;
+          if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
-        ptx::wgmma_commit();
-        // keep one group in flight: the previous k-block's group has retired, its stage is free
-        ptx::wgmma_wait<1>();
-        if (kb > 0 && lane == 0) {
+        ptx::wgmma_wait<0>();
+        if (lane == 0) {
           ptx::mbar_arrive(empty_bar(prev));
           if (CG == 2) ptx::mbar_arrive_cluster(empty_bar(prev), peer);
         }
-        prev = stage;
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
-      }
-      ptx::wgmma_wait<0>();
-      if (lane == 0) {
-        ptx::mbar_arrive(empty_bar(prev));
-        if (CG == 2) ptx::mbar_arrive_cluster(empty_bar(prev), peer);
+      };
+      if (KIND == ptx::KIND_TF32 && half_tile(tc)) {
+        mainloop(std::integral_constant<int, ptx::KIND_F16>{}, num_kb16);
+      } else {
+        mainloop(std::integral_constant<int, KIND>{}, num_kb);
       }
 
       // ---- epilogue: this warp's 16 rows x BN columns ----
@@ -415,16 +449,18 @@ __device__ __forceinline__ void gemm_wgmma_body(const CUtensorMap &tmap_a, const
 template <int KIND, typename TOut, int CG, int BN>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                  const __grid_constant__ CUtensorMap tmap_a16, const __grid_constant__ CUtensorMap tmap_b16,
                   const __grid_constant__ CUtensorMap tmap_c, TOut *__restrict__ C, const GemmParams p) {
-  gemm_wgmma_body<KIND, TOut, CG, BN, false>(tmap_a, tmap_b, tmap_c, C, p);
+  gemm_wgmma_body<KIND, TOut, CG, BN, false>(tmap_a, tmap_b, tmap_a16, tmap_b16, tmap_c, C, p);
 }
 
 // C <- C + A'B'^T (mm_kernel_enqueue_accumulate); instantiated in gemm_wgmma_acc.cu only.
 template <int KIND, typename TOut, int CG, int BN>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_wgmma_accumulate_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                             const __grid_constant__ CUtensorMap tmap_a16, const __grid_constant__ CUtensorMap tmap_b16,
                              const __grid_constant__ CUtensorMap tmap_c, TOut *__restrict__ C, const GemmParams p) {
-  gemm_wgmma_body<KIND, TOut, CG, BN, true>(tmap_a, tmap_b, tmap_c, C, p);
+  gemm_wgmma_body<KIND, TOut, CG, BN, true>(tmap_a, tmap_b, tmap_a16, tmap_b16, tmap_c, C, p);
 }
 
 // ---- host side -----------------------------------------------------------------------------------
@@ -490,6 +526,7 @@ int num_sms() {
 
 struct LaunchPlan {
   const CUtensorMap *map_a, *map_b, *map_c;
+  const CUtensorMap *map_a16, *map_b16;  // float's fp16 operand copies; map_a / map_b again for the other types
   void *c;
   GemmParams p;
   int requested_stages;
@@ -531,7 +568,8 @@ int launch_gemm_variant(LaunchPlan plan) {
   cfg.attrs = attr;
   cfg.numAttrs = 1;
   if (plan.p.tile_sync) MM_CUDA_TRY(cudaMemsetAsync(plan.p.tile_sync, 0, sizeof(unsigned int), plan.stream));
-  MM_CUDA_TRY(cudaLaunchKernelEx(&cfg, kern, *plan.map_a, *plan.map_b, *plan.map_c, static_cast<TOut *>(plan.c), plan.p));
+  MM_CUDA_TRY(cudaLaunchKernelEx(&cfg, kern, *plan.map_a, *plan.map_b, *plan.map_a16, *plan.map_b16, *plan.map_c,
+                                 static_cast<TOut *>(plan.c), plan.p));
   return MM_OK;
 }
 
@@ -549,22 +587,31 @@ int dispatch_variant(int cg, int bn, const LaunchPlan &plan) {
 }
 
 // The tensor maps and run-time parameters of one GEMM launch: everything but the kernel variant.  `maps`
-// (A, B, C) must outlive the launch; `k` is the K extent the operands carry.
+// (A, B, C, fp16 A, fp16 B) must outlive the launch; `k` is the K extent the operands carry.  `half`: float's fp16
+// operand copies and fits flags (gemm_tcgen05.cu), or empty.
 int plan_gemm(int dtype, const void *a_op, const void *b_op, void *c, unsigned rows, unsigned k, unsigned m,
               const Tuning &t, unsigned int *tile_sync, const unsigned int *b_ready, unsigned b_ready_target,
-              bool attributes_only, cudaStream_t stream, const GemmBatch &batch, CUtensorMap (&maps)[3],
-              LaunchPlan *plan) {
+              bool attributes_only, cudaStream_t stream, const GemmBatch &batch, const HalfOperands &half,
+              CUtensorMap (&maps)[5], LaunchPlan *plan) {
   const size_t eb = elem_bytes(dtype);
   const int cg = t.cta_group(), bn = t.block_n();
+  const bool use_half = dtype == MM_DTYPE_FLOAT && half.fits_a != nullptr;
   if (batch.count > 1 && b_ready != nullptr) return fail(MM_ERR_UNSUPPORTED, "batched calls need a complete B operand");
   std::memset(&maps[2], 0, sizeof(maps[2]));
-  *plan = LaunchPlan{&maps[0], &maps[1], &maps[2], c, {}, t.stages(), attributes_only, stream};
+  *plan = LaunchPlan{&maps[0], &maps[1], &maps[2], use_half ? &maps[3] : &maps[0], use_half ? &maps[4] : &maps[1],
+                     c, {}, t.stages(), attributes_only, stream};
   if (!attributes_only) {
     // the problems of a batch stacked along the rows (one copy when the operand is shared)
     int rc = make_operand_map(&maps[0], a_op, dtype, uint64_t(batch.a_copies()) * rows, k, BLOCK_M);
     if (rc != MM_OK) return rc;
     rc = make_operand_map(&maps[1], b_op, dtype, uint64_t(batch.b_copies()) * m, k, uint32_t(bn / cg));
     if (rc != MM_OK) return rc;
+    if (use_half) {
+      rc = make_operand_map(&maps[3], half.a, MM_DTYPE_HALF, uint64_t(batch.a_copies()) * rows, k, BLOCK_M);
+      if (rc != MM_OK) return rc;
+      rc = make_operand_map(&maps[4], half.b, MM_DTYPE_HALF, uint64_t(batch.b_copies()) * m, k, uint32_t(bn / cg));
+      if (rc != MM_OK) return rc;
+    }
     if (t.tma_store()) {
       rc = make_c_map(&maps[2], c, dtype, rows, m, batch.count);
       if (rc != MM_OK) return rc;
@@ -583,6 +630,8 @@ int plan_gemm(int dtype, const void *a_op, const void *b_op, void *c, unsigned r
   p.l2_policy = t.l2_policy() == 1 ? ptx::L2_EVICT_FIRST : (t.l2_policy() == 2 ? ptx::L2_EVICT_LAST : ptx::L2_EVICT_NORMAL);
   p.tile_sync = t.tile_sync() ? tile_sync : nullptr;
   p.b_ready = b_ready;
+  p.fits_a = use_half ? half.fits_a : nullptr;
+  p.fits_b = use_half ? half.fits_b : nullptr;
   return MM_OK;
 }
 
@@ -598,6 +647,7 @@ int wgmma_bf16_gemm(const void *a_op, const void *b_op, void *c, unsigned rows, 
 // live in gemm_wgmma_acc.cu.  `k` is the K extent the operands carry (3K for 3xTF32).
 int wgmma_accumulate_gemm(int dtype, const void *a_op, const void *b_op, void *c, unsigned rows, unsigned k, unsigned m,
                           const Tuning &t, unsigned int *tile_sync, const unsigned int *b_ready,
-                          unsigned b_ready_target, bool attributes_only, cudaStream_t stream, const GemmBatch &batch);
+                          unsigned b_ready_target, bool attributes_only, cudaStream_t stream, const GemmBatch &batch,
+                          const HalfOperands &half);
 
 }  // namespace mm
