@@ -5,7 +5,7 @@ Everything here takes torch tensors on any device, so the CPU suite (tests/test_
 code on small shapes.
 
 * `exact_operands`: the exact data of tensor_numerics.full_size_scheme, drawn with a seeded torch.Generator in row
-  blocks on the given device.
+  blocks on the given device; "tf32" with A's last row times 2^20, so that float runs on TF32, "tf32h" without.
 * `fp64_reference`: the FP64 product in row blocks of A, stored once in the output type (modulo 256 for uint8).
 * `min_plus_reference`, `sequential_half_reference`: Naive<>'s order of operations for (Add, Min) and half
   (Multiply, Add), one torch op per Map and per Reduce, each rounding once.
@@ -143,9 +143,11 @@ def check_guard(torch, what, guard, poison):
 
 def exact_operands(torch, path, n, k, m, seed, device, row_block=ROW_BLOCK):
     """A (n x k) and B (k x m) of path's exact data (tensor_numerics.full_size_scheme), in its input type on
-    `device`.  uint8: full-range bytes.  Adjacent rows of A and adjacent columns of B never share a scale."""
-    dt = {"tf32": torch.float32, "tf32x3": torch.float32, "f16": torch.float16, "bf16": torch.bfloat16,
-          "dmma": torch.float64, "u8": torch.uint8}[path]
+    `device`.  uint8: full-range bytes.  Adjacent rows of A and adjacent columns of B never share a scale.  "tf32":
+    the "tf32h" data with A's last row times tensor_numerics.PLANT_SCALE (exact; its values are no halves, so the
+    float GEMM runs on TF32)."""
+    dt = {"tf32": torch.float32, "tf32h": torch.float32, "tf32x3": torch.float32, "f16": torch.float16,
+          "bf16": torch.bfloat16, "dmma": torch.float64, "u8": torch.uint8}[path]
     g = torch.Generator(device=device)
     g.manual_seed(seed)
     if path == "u8":
@@ -171,14 +173,16 @@ def exact_operands(torch, path, n, k, m, seed, device, row_block=ROW_BLOCK):
     col_scale = torch.exp2(eb.to(wide))[None, :]
     a = fill(torch.empty((n, k), device=device, dtype=dt), k, lambda r0, r1: torch.exp2(ea[r0:r1].to(wide))[:, None])
     b = fill(torch.empty((k, m), device=device, dtype=dt), m, lambda r0, r1: col_scale)
+    if path == "tf32":
+        a[n - 1] *= tn.PLANT_SCALE
     return a, b
 
 
 def fp64_reference(torch, path, a, b, row_block=ROW_BLOCK):
     """C = A B evaluated in FP64 (exact for the exact data), stored once in path's output type: float32 for the TF32
     paths, FP64 -> float32 (exact) -> half / bfloat16, float64 for DMMA, the exact sum modulo 256 for uint8."""
-    out = {"tf32": torch.float32, "tf32x3": torch.float32, "f16": torch.float16, "bf16": torch.bfloat16,
-           "dmma": torch.float64, "u8": torch.uint8}[path]
+    out = {"tf32": torch.float32, "tf32h": torch.float32, "tf32x3": torch.float32, "f16": torch.float16,
+           "bf16": torch.bfloat16, "dmma": torch.float64, "u8": torch.uint8}[path]
     b64 = b.to(torch.float64)
     c = torch.empty((a.shape[0], b.shape[1]), device=a.device, dtype=out)
     for r0 in range(0, a.shape[0], row_block):

@@ -11,7 +11,11 @@
   prepared operands, and of DMMA against an FP64 reference that carries error itself.
 * `ieee_reference`: an elementwise FP64 evaluation (no BLAS, which may skip zero multipliers and hide inf * 0).
 
-Paths: "tf32", "tf32x3", "f16", "bf16", "dmma" (double), "u8".  bfloat16 values are np.uint16 bit patterns.
+Paths: "tf32", "tf32h", "tf32x3", "f16", "bf16", "dmma" (double), "u8".  bfloat16 values are np.uint16 bit patterns.
+"tf32" and "tf32h" are float (Multiply, Add) on its two datapaths: a problem whose TF32-rounded A and B all fit a half
+(`fits_half`, gemm_hls_b200/csrc/fits_half.h) runs on the f16 wgmma, any other on TF32.  They share the type, the
+preparation and the bound; only the exact data differs: "tf32h" fits, and "tf32" is the same data with one row of A
+per problem times 2^20 (`PLANT_SCALE`), which no half holds.
 """
 import math
 
@@ -19,12 +23,13 @@ import numpy as np
 
 import bf16_naive
 
-PATHS = ("tf32", "tf32x3", "f16", "bf16", "dmma", "u8")
+PATHS = ("tf32", "tf32h", "tf32x3", "f16", "bf16", "dmma", "u8")
+FLOAT_PATHS = ("tf32", "tf32h", "tf32x3")
 TF32_MAX_BITS = 0x7F7FE000          # the largest finite TF32 value (10 explicit mantissa bits)
 FLT_MAX = float(np.finfo(np.float32).max)
 
 # Integer magnitudes that the input type holds exactly, and that leave TF32 rounding the identity (so lo = 0).
-TYPE_INT_LIMIT = {"tf32": 1024, "tf32x3": 1024, "f16": 2048, "bf16": 256, "dmma": 1024}
+TYPE_INT_LIMIT = {"tf32": 1024, "tf32h": 1024, "tf32x3": 1024, "f16": 2048, "bf16": 256, "dmma": 1024}
 EXACT_S_LIMIT = 2 ** 22
 
 # alpha_path of check_bound: |c - r| <= half an ulp + alpha * K_eff * 2^-23 * S.  alpha = 1 bounds any order of
@@ -34,7 +39,12 @@ EXACT_S_LIMIT = 2 ** 22
 # simulated round-toward-zero accumulation in random order needs (<= 0.19 on same-sign data,
 # tests/test_tensor_numerics_cpu.py).  Worst seen on the H100, all on same-sign data:
 #   tf32 0.0654, tf32x3 0.0416, f16 0.0534, bf16 0.0391.
-ALPHA = {"tf32": 0.3, "tf32x3": 0.25, "f16": 0.25, "bf16": 0.25}
+ALPHA = {"tf32": 0.3, "tf32h": 0.3, "tf32x3": 0.25, "f16": 0.25, "bf16": 0.25}
+
+# One row of A per problem of "tf32" exact data is scaled by this: its values are >= 2^16, TF32-exact but no half, so
+# the problem runs on TF32.  Every C element of that row is still one integer <= 2^22 times one power of two (<= 2^41),
+# exact in FP32; sent to the f16 datapath by mistake, the row's fp16 copy is +-inf and C holds inf or NaN there.
+PLANT_SCALE = 2.0 ** 20
 
 
 # ---- operand preparation --------------------------------------------------------------------------------------
@@ -76,6 +86,25 @@ def split_tf32(x):
     return hi, np.where(np.isinf(x), np.float32(0), lo).astype(np.float32)
 
 
+def fits_half_each(x):
+    """Elementwise gemm_hls_b200/csrc/fits_half.h on rna_tf32(x): the rounded value is +-0 or a normal half
+    (2^-14 <= |v| < 2^16, biased float exponent 113 .. 142)."""
+    u = rna_tf32(x).view(np.uint32)
+    e = (u >> np.uint32(23)) & np.uint32(0xFF)
+    return ((u & np.uint32(0x7FFFFFFF)) == 0) | ((e >= 113) & (e <= 142))
+
+
+def fits_half(x):
+    """Whether an operand sends its float problem to the f16 datapath: every TF32-rounded value is +-0 or a normal
+    half.  A problem runs on f16 when both its A and its B fit."""
+    return bool(np.all(fits_half_each(x)))
+
+
+def datapath(a, b):
+    """"tf32h" when the float problem (a, b) runs on the f16 wgmma, "tf32" when it runs on TF32."""
+    return "tf32h" if fits_half(a) and fits_half(b) else "tf32"
+
+
 def finite_or_zero(hi):
     """The hi of the 3xTF32 cross terms: +-inf replaced by 0, so that hi * hi alone carries infinities."""
     return np.where(np.isinf(hi), np.float32(0), hi).astype(np.float32)
@@ -95,7 +124,7 @@ def prepared_operands(path, a, b, transposed_a=False):
     a = np.asarray(a)
     if transposed_a:
         a = a.T
-    if path == "tf32":
+    if path in ("tf32", "tf32h"):
         return rna_tf32(a).astype(np.float64), rna_tf32(b).astype(np.float64)
     if path == "tf32x3":
         ha, la = split_tf32(a)
@@ -127,7 +156,8 @@ def ieee_reference(ap, bp):
 # ---- output types ---------------------------------------------------------------------------------------------
 
 # (mantissa bits, smallest normal exponent) of each path's output type
-_OUT_FORMAT = {"tf32": (23, -126), "tf32x3": (23, -126), "f16": (10, -14), "bf16": (7, -126), "dmma": (52, -1022)}
+_OUT_FORMAT = {"tf32": (23, -126), "tf32h": (23, -126), "tf32x3": (23, -126), "f16": (10, -14), "bf16": (7, -126),
+               "dmma": (52, -1022)}
 
 
 def half_ulp(path, x):
@@ -142,7 +172,7 @@ def store(path, exact):
     """The exact float64 C stored once in the output type (round to nearest even), as the kernel's epilogue does;
     uint8: modulo 256."""
     exact = np.asarray(exact, np.float64)
-    if path in ("tf32", "tf32x3"):
+    if path in FLOAT_PATHS:
         return exact.astype(np.float32)
     if path == "f16":
         return exact.astype(np.float16)
@@ -238,12 +268,12 @@ def exact_limit(path, k):
 # 2^ea per row of A and 2^eb per column of B, ea and eb cycling through these inclusive ranges.  Every C element is
 # then an integer of magnitude <= limit^2 K times the one power of two 2^(ea + eb) of its row and column.  half:
 # |C| <= 2^22 2^(-4 - 3) < 2^15, and every nonzero |C| >= 2^(-6 - 6) = 2^-12, a normal half.
-_FULL_SIZE_EXP = {"tf32": ((-3, -1), (-2, 0)), "tf32x3": ((-3, -1), (-2, 0)), "f16": ((-6, -4), (-6, -3)),
-                  "bf16": ((-3, -1), (-2, 0)), "dmma": ((-3, -1), (-2, 0))}
+_FULL_SIZE_EXP = {"tf32": ((-3, -1), (-2, 0)), "tf32h": ((-3, -1), (-2, 0)), "tf32x3": ((-3, -1), (-2, 0)),
+                  "f16": ((-6, -4), (-6, -3)), "bf16": ((-3, -1), (-2, 0)), "dmma": ((-3, -1), (-2, 0))}
 # Bound on limit^2 K: the FP32-accumulating paths keep 2 bits of FP32's 24 to spare (EXACT_S_LIMIT); DMMA
 # accumulates in FP64 and keeps the same 2 bits of FP64's 53, so it takes the type's whole exact range (1024).
-FULL_SIZE_S_LIMIT = {"tf32": EXACT_S_LIMIT, "tf32x3": EXACT_S_LIMIT, "f16": EXACT_S_LIMIT, "bf16": EXACT_S_LIMIT,
-                     "dmma": 2 ** 51}
+FULL_SIZE_S_LIMIT = {"tf32": EXACT_S_LIMIT, "tf32h": EXACT_S_LIMIT, "tf32x3": EXACT_S_LIMIT, "f16": EXACT_S_LIMIT,
+                     "bf16": EXACT_S_LIMIT, "dmma": 2 ** 51}
 
 
 def full_size_scheme(path, k):
@@ -263,7 +293,7 @@ def _nonzero_ints(rng, lim, shape):
 
 
 def _in_dtype(path, x):
-    if path in ("tf32", "tf32x3"):
+    if path in FLOAT_PATHS:
         return x.astype(np.float32)
     if path == "f16":
         return x.astype(np.float16)
@@ -272,10 +302,24 @@ def _in_dtype(path, x):
     return x.astype(np.float64)
 
 
-def exact_operands(path, n, k, m, batch=1, seed=0, shared_a=False, shared_b=False):
+def plant_rows(path, n, copies, first="first"):
+    """The row of each of A's copies that "tf32" data scales by PLANT_SCALE (None for every other path): copy 0 at
+    its first row (`first` "first") or its last ("last"), then alternating, and in a batch the last copy always at
+    its last row."""
+    if path != "tf32":
+        return [None] * copies
+    rows = [0 if (i % 2 == 0) == (first == "first") else n - 1 for i in range(copies)]
+    if copies > 1:
+        rows[-1] = n - 1
+    return rows
+
+
+def exact_operands(path, n, k, m, batch=1, seed=0, shared_a=False, shared_b=False, plant="first"):
     """A (batch_a x n x k) and B (batch_b x k x m) of exact data for `path`, in its input type (batch_x = 1 when
     shared).  uint8: full-range bytes (the integer accumulation is exact for any data).  Asserts the exactness
-    precondition S <= 2^22 (over the integers) and that every value and every C is a normal number of the type."""
+    precondition S <= 2^22 (over the integers) and that every value and every C is a normal number of the type.
+    "tf32": one row of each copy of A times PLANT_SCALE (plant_rows, `plant` the first copy's row), so that every
+    problem runs on TF32; "tf32h": the same data without it, every problem on f16 (both asserted with fits_half)."""
     rng = np.random.default_rng(seed)
     ba, bb = (1 if shared_a else batch), (1 if shared_b else batch)
     if path == "u8":
@@ -298,7 +342,13 @@ def exact_operands(path, n, k, m, batch=1, seed=0, shared_a=False, shared_b=Fals
     if path == "f16":   # every operand and every C a normal half
         assert EXACT_S_LIMIT * 2.0 ** emax < 65504 and emin >= -14
         assert np.abs(a).min() >= 2.0 ** -14 and np.abs(b).min() >= 2.0 ** -14
-    return _in_dtype(path, a), _in_dtype(path, b)
+    for i, r in enumerate(plant_rows(path, n, ba, plant)):
+        if r is not None:
+            a[i, r, :] *= PLANT_SCALE
+    a, b = _in_dtype(path, a), _in_dtype(path, b)
+    if path in ("tf32", "tf32h"):
+        assert all(datapath(a[i if ba > 1 else 0], b[i if bb > 1 else 0]) == path for i in range(batch))
+    return a, b
 
 
 def tie_operands(route, n, k, m, seed=0):

@@ -66,6 +66,22 @@ def test_predicate_is_exact_normal_half_round_trip(fits, sign):
     assert np.all((exact & ~got) == (exact & ~normal_or_zero))           # only the half-subnormal band is left out
 
 
+@pytest.mark.parametrize("sign", [0, 1])
+def test_numpy_restatement_matches_the_predicate(fits, sign):
+    """tensor_numerics.fits_half_each (on rna_tf32 of its input) against the compiled predicate on every TF32 bit
+    pattern of one sign, infinities and NaN included, and on floats whose rounding crosses the boundary."""
+    import tensor_numerics as tn
+    bits = (np.uint32(sign) << np.uint32(31)) | (np.arange(1 << 18, dtype=np.uint32) << np.uint32(13))
+    assert np.array_equal(tn.fits_half_each(bits.view(np.float32)), fits(bits))
+    # every float32 just below and above each TF32 value: the predicate of the rounded value
+    near = np.concatenate([bits - np.uint32(1), bits + np.uint32(0xFFF), bits + np.uint32(0x1000)])
+    near = near[(near >> np.uint32(31)) == sign].view(np.float32)
+    with np.errstate(invalid="ignore"):
+        rounded = tn.rna_tf32(near).view(np.uint32)
+    assert np.array_equal(tn.fits_half_each(near), fits(rounded))
+    assert tn.fits_half(np.float32([0.0, -0.0, 9.99, 65504.0])) and not tn.fits_half(np.float32([1.0, 65520.0]))
+
+
 @pytest.mark.parametrize("x,want", [(0.0, True), (-0.0, True), (2.0 ** -14, True), (2.0 ** -15, False),
                                     (65504.0, True), (65536.0, False), (1e-40, False), (np.inf, False),
                                     (-np.inf, False), (np.nan, False), (9.99, True)])

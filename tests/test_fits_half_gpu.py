@@ -11,6 +11,7 @@ import pytest
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import tensor_numerics as tn  # noqa: E402
+import test_float_datapaths_gpu as fd  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 
@@ -143,21 +144,5 @@ def test_fitting_problems_run_on_the_f16_datapath(torch, mm):
     """On operands that are exactly halves the rounding is the identity, so tf32_no_round = 1 multiplies the same
     values on the TF32 datapath.  Same-sign data: the f16 datapath rounds its partial sums differently from TF32
     (DESIGN.md §3.1), so a fitting problem gives other bits than TF32, and the same problem with one value of 2^16
-    in A (not a half, but TF32-exact) gives exactly TF32's bits."""
-    n, k, m = 256, 1024, 256
-    rng = np.random.default_rng(5)
-    a = rng.uniform(1, 10, (n, k)).astype(np.float16).astype(np.float32)
-    b = rng.uniform(1, 10, (k, m)).astype(np.float16).astype(np.float32)
-    a_out = a.copy()
-    a_out[n - 1, k - 1] = 2.0 ** 16
-
-    def run(x, no_round):
-        ctx = mm.Context(0)
-        ctx.set_tuning(tf32_no_round=no_round)
-        c = _single(torch, mm, ctx, x, b)
-        ctx.close()
-        return c
-    fit, fit_tf32 = run(a, 0), run(a, 1)
-    assert np.mean(fit.view(np.uint32) == fit_tf32.view(np.uint32)) < 0.5
-    tn.check_bound("tf32", fit, *tn.prepared_product("tf32", a, b), k)
-    assert _same(run(a_out, 0), run(a_out, 1))
+    in A (not a half, but TF32-exact) gives exactly TF32's bits (test_float_datapaths_gpu.check_probe_datapaths)."""
+    fd.check_probe_datapaths(torch, mm)

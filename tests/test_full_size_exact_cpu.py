@@ -56,7 +56,7 @@ def test_full_size_scheme_data_on_small_shapes():
     """exact_operands draws nonzero integers within the limit times the cycling row / column scales, and the
     FP64 reference is the exact product, stored in each output type."""
     n, k, m = 37, 64, 45
-    for path in ("tf32", "f16", "bf16", "dmma"):
+    for path in ("tf32h", "f16", "bf16", "dmma"):
         a, b = fc.exact_operands(torch, path, n, k, m, seed=3, device="cpu", row_block=16)
         lim, (ea0, ea1), (eb0, eb1) = tn.full_size_scheme(path, k)
         a64, b64 = a.to(torch.float64), b.to(torch.float64)
@@ -67,6 +67,14 @@ def test_full_size_scheme_data_on_small_shapes():
         want = fc.fp64_reference(torch, path, a, b, row_block=16)
         exact = (a64.numpy() @ b64.numpy())
         np.testing.assert_array_equal(want.to(torch.float64).numpy(), tn.to_float64(path, tn.store(path, exact)))
+    # "tf32": the "tf32h" data with A's last row times 2^20; only that row of the exact C changes, by that power of two
+    a, b = fc.exact_operands(torch, "tf32", n, k, m, seed=3, device="cpu", row_block=16)
+    ah, bh = fc.exact_operands(torch, "tf32h", n, k, m, seed=3, device="cpu", row_block=16)
+    assert torch.equal(b, bh) and torch.equal(a[:-1], ah[:-1]) and torch.equal(a[-1], ah[-1] * tn.PLANT_SCALE)
+    assert tn.datapath(a.numpy(), b.numpy()) == "tf32" and tn.datapath(ah.numpy(), bh.numpy()) == "tf32h"
+    want = fc.fp64_reference(torch, "tf32", a, b, row_block=16)
+    exact = a.to(torch.float64).numpy() @ b.to(torch.float64).numpy()
+    np.testing.assert_array_equal(want.to(torch.float64).numpy(), exact)
     a, b = fc.exact_operands(torch, "u8", n, k, m, seed=3, device="cpu")
     want = fc.fp64_reference(torch, "u8", a, b, row_block=16)
     exact = a.numpy().astype(np.int64) @ b.numpy().astype(np.int64)

@@ -103,7 +103,8 @@ def _run_settings(torch, mm, settings, a, b, want, locate_for, dtype, mp, rd, mo
 def _tensor_core_case(torch, mm, path, n, settings, seed, poisons=(0xFF,)):
     a, b = fc.exact_operands(torch, path, n, n, n, seed, "cuda")
     want = fc.fp64_reference(torch, path, a, b)
-    dtype = {"tf32": mm.FLOAT, "f16": mm.HALF, "bf16": mm.BFLOAT16, "u8": mm.UINT8, "dmma": mm.DOUBLE}[path]
+    dtype = {"tf32": mm.FLOAT, "tf32h": mm.FLOAT, "f16": mm.HALF, "bf16": mm.BFLOAT16, "u8": mm.UINT8,
+             "dmma": mm.DOUBLE}[path]
     if path == "dmma":
         sms = _sms(torch)
         locate_for = lambda knobs: fc.grid_locator("gemm_dmma_tma_kernel", fc.dmma_tile_rows(
@@ -114,10 +115,17 @@ def _tensor_core_case(torch, mm, path, n, settings, seed, poisons=(0xFF,)):
 
 
 def test_float_16384_tf32_and_3xtf32_exact(torch, mm):
-    """bench.py float16384, the headline: TF32 wgmma, and the same data under MM_FLAG_TF32X3."""
+    """bench.py float16384, the headline: data that fits a half, on the f16 datapath of the float wgmma GEMM, and the
+    same data under MM_FLAG_TF32X3."""
     assert mm.kernel_path(mm.FLOAT) == "wgmma_tf32"
-    _tensor_core_case(torch, mm, "tf32", 16384, [("float 16384^3 tf32", {}, 0),
-                                                 ("float 16384^3 3xtf32", {}, mm.FLAG_TF32X3)], seed=41)
+    _tensor_core_case(torch, mm, "tf32h", 16384, [("float 16384^3 f16 datapath", {}, 0),
+                                                  ("float 16384^3 3xtf32", {}, mm.FLAG_TF32X3)], seed=41)
+
+
+def test_float_16384_tf32_datapath_exact(torch, mm):
+    """bench.py float16384 on the TF32 datapath: the same kind of data with A's last row times 2^20, which no half
+    holds."""
+    _tensor_core_case(torch, mm, "tf32", 16384, [("float 16384^3 tf32 datapath", {}, 0)], seed=41)
 
 
 def test_half_32768_f16_exact(torch, mm):
@@ -186,8 +194,8 @@ def test_half_8192_exact_flag_packed_bit_exact(torch, mm):
 # ---- host-pointer entries ---------------------------------------------------------------------------------------
 
 def _host_case(torch, n, seed):
-    a, b = fc.exact_operands(torch, "tf32", n, n, n, seed, "cuda")
-    want = fc.fp64_reference(torch, "tf32", a, b)
+    a, b = fc.exact_operands(torch, "tf32h", n, n, n, seed, "cuda")
+    want = fc.fp64_reference(torch, "tf32h", a, b)
     return a.cpu().numpy(), b.cpu().numpy(), want
 
 

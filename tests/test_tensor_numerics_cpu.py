@@ -114,9 +114,15 @@ def test_split_tf32_infinities_and_nan():
 # ---- generators --------------------------------------------------------------------------------------------------
 
 def _gpu_exact_shapes():
-    cases = [(p, s, 1) for p, s in gpu.MULTIWAVE.items()]
-    cases += [(p, (1, w, w), 1) for p, w in gpu.WIDTH.items()] + [(p, (129, 3 * w, 17 * w), 1) for p, w in gpu.WIDTH.items()]
-    cases += [(p, s, 9) for p, s in gpu.BATCHED.items()]
+    """Every exact case of the GPU file; the f16-datapath float data ("tf32h") last, after the cases of the other
+    paths in their own order."""
+    cases = []
+    for last in (False, True):
+        keep = lambda p: (p == "tf32h") == last
+        cases += [(p, s, 1) for p, s in gpu.MULTIWAVE.items() if keep(p)]
+        cases += [(p, (1, w, w), 1) for p, w in gpu.WIDTH.items() if keep(p)]
+        cases += [(p, (129, 3 * w, 17 * w), 1) for p, w in gpu.WIDTH.items() if keep(p)]
+        cases += [(p, s, 9) for p, s in gpu.BATCHED.items() if keep(p)]
     return cases
 
 
@@ -137,7 +143,7 @@ def test_exact_generator_precondition(path, shape, batch):
         e = np.floor(np.log2(np.abs(x)))
         frac = np.abs(x) / np.exp2(e)
         assert np.all(frac * 2 ** 12 == np.round(frac * 2 ** 12))
-    if path in ("tf32", "tf32x3"):
+    if path in tn.FLOAT_PATHS:
         assert np.array_equal(tn.rna_tf32(a), a) and np.array_equal(tn.split_tf32(b)[1], np.zeros_like(b))
     s_int = np.abs(np.round(a64 / _row_scale(a64))) @ np.abs(np.round(b64 / _col_scale(b64)))
     assert s_int.max() <= tn.EXACT_S_LIMIT

@@ -6,6 +6,9 @@ a. Operand preparation bit for bit through identity products (C = A' I), on ever
 b. Zero-tolerance products on multi-wave schedules: every CTA group runs several tiles, the last wave is partial,
    the rasterisation has a tail group and there are more k-blocks than ring stages; every tuning variant.
 c. Batched calls over several waves, each problem against its own exact product.
+   Float runs b and c, the edge shapes and the TF32 ties on both of its datapaths: "tf32h" data fits a half and runs
+   on the f16 wgmma, "tf32" data carries a row of A times 2^20 and runs on TF32 (tensor_numerics.exact_operands).
+   Each call asserts on the host which of the two its operands take.
 d. Per-element error bounds on random data (same-sign, mixed-sign, exponent-spread; long K).
 e. +-inf, NaN and near-overflow operands: the class of every element as IEEE arithmetic on the prepared operands.
 
@@ -25,14 +28,14 @@ import tensor_numerics as tn  # noqa: E402
 pytestmark = pytest.mark.gpu
 
 GUARD = 4096
-WGMMA_PATHS = ("tf32", "tf32x3", "f16", "bf16", "u8")
+WGMMA_PATHS = ("tf32", "tf32h", "tf32x3", "f16", "bf16", "u8")
 
 # One shape per family that takes every scheduler path under the default tuning (CG 2, BN 256, raster 2048 rows):
 # float: 10 x 18 = 180 tiles on 66 CTA groups (raster groups of 8 + 2 row tiles); with CG 1, BN 128: 19 x 35 = 665
 # tiles on 132 CTAs (groups of 16 + 3).  The other families hold the same tile counts at their memory width.
-MULTIWAVE = {"tf32": (2305, 272, 4368), "tf32x3": (2305, 272, 4368), "f16": (2305, 544, 4384),
-             "bf16": (2305, 544, 4384), "u8": (2305, 576, 4416), "dmma": (2305, 264, 4360)}
-WIDTH = {"tf32": 16, "tf32x3": 16, "f16": 32, "bf16": 32, "u8": 64, "dmma": 8}
+MULTIWAVE = {"tf32": (2305, 272, 4368), "tf32h": (2305, 272, 4368), "tf32x3": (2305, 272, 4368),
+             "f16": (2305, 544, 4384), "bf16": (2305, 544, 4384), "u8": (2305, 576, 4416), "dmma": (2305, 264, 4360)}
+WIDTH = {"tf32": 16, "tf32h": 16, "tf32x3": 16, "f16": 32, "bf16": 32, "u8": 64, "dmma": 8}
 
 # tuning variants: (knobs, transposed A); raster_rows 768 makes CG 2 groups of 3 + 3 + 3 + 1 row tiles
 VARIANTS = ([(dict(cta_group=cg, block_n=bn, tma_store=ts), False) for cg in (1, 2) for bn in (128, 256)
@@ -63,13 +66,13 @@ def ctx(mm):
 
 
 def _mm_dtype(mm, path):
-    return {"tf32": mm.FLOAT, "tf32x3": mm.FLOAT, "f16": mm.HALF, "bf16": mm.BFLOAT16, "dmma": mm.DOUBLE,
-            "u8": mm.UINT8}[path]
+    return {"tf32": mm.FLOAT, "tf32h": mm.FLOAT, "tf32x3": mm.FLOAT, "f16": mm.HALF, "bf16": mm.BFLOAT16,
+            "dmma": mm.DOUBLE, "u8": mm.UINT8}[path]
 
 
 def _torch_dtype(torch, path):
-    return {"tf32": torch.float32, "tf32x3": torch.float32, "f16": torch.float16, "bf16": torch.bfloat16,
-            "dmma": torch.float64, "u8": torch.uint8}[path]
+    return {"tf32": torch.float32, "tf32h": torch.float32, "tf32x3": torch.float32, "f16": torch.float16,
+            "bf16": torch.bfloat16, "dmma": torch.float64, "u8": torch.uint8}[path]
 
 
 def _dev(torch, path, x):
@@ -96,7 +99,7 @@ def _gpu_matmul(torch):
 def _run(torch, mm, ctx, path, a, b, n, k, m, flags=0, batch=None, poison=0xFF):
     """C of one call (batch=None) or one batched call on device operands a, b, into a poisoned buffer; checks the
     guard and that C holds no poison.  Returns C on the host, shaped (batch,) n x m."""
-    item = {"tf32": 4, "tf32x3": 4, "f16": 2, "bf16": 2, "dmma": 8, "u8": 1}[path]
+    item = {"tf32": 4, "tf32h": 4, "tf32x3": 4, "f16": 2, "bf16": 2, "dmma": 8, "u8": 1}[path]
     nbytes = (batch or 1) * n * m * item
     raw = torch.full((nbytes + GUARD,), poison, dtype=torch.uint8, device="cuda")
     c = raw[:nbytes].view(_torch_dtype(torch, path))
@@ -123,14 +126,14 @@ def _poisons(path):
 _EXACT_CACHE = {}
 
 
-def _exact_case(torch, path, n, k, m, seed, batch=1, shared_a=False, shared_b=False):
+def _exact_case(torch, path, n, k, m, seed, batch=1, shared_a=False, shared_b=False, plant="first"):
     """Exact operands (host) and the exact C stored in the output type, from an FP64 product on the GPU (exact for
-    integer data)."""
-    key = (path, n, k, m, seed, batch, shared_a, shared_b)
+    integer data).  `plant`: where "tf32" data puts its row times 2^20 (tensor_numerics.plant_rows)."""
+    key = (path, n, k, m, seed, batch, shared_a, shared_b, plant)
     if key not in _EXACT_CACHE:
         if len(_EXACT_CACHE) > 4:
             _EXACT_CACHE.clear()
-        a, b = tn.exact_operands(path, n, k, m, batch, seed, shared_a, shared_b)
+        a, b = tn.exact_operands(path, n, k, m, batch, seed, shared_a, shared_b, plant)
         c64 = torch.matmul(torch.from_numpy(tn.to_float64(path, a)).cuda(),
                            torch.from_numpy(tn.to_float64(path, b)).cuda()).cpu().numpy()
         _EXACT_CACHE[key] = (a, b, tn.store(path, c64))
@@ -220,9 +223,16 @@ def test_subnormal_operands(torch, mm, ctx, path):
 
 # ---- b. zero-tolerance products on multi-wave schedules ---------------------------------------------------------
 
-def _exact_call(torch, mm, ctx, path, n, k, m, seed, transposed=False):
-    a, b, want = _exact_case(torch, path, n, k, m, seed)
+def _assert_datapath(path, a, b):
+    """Float: the operands take the datapath that the path key names (a fitting problem runs on the f16 wgmma)."""
+    if path in ("tf32", "tf32h"):
+        assert tn.datapath(a, b) == path, "%s data that runs on the %s datapath" % (path, tn.datapath(a, b))
+
+
+def _exact_call(torch, mm, ctx, path, n, k, m, seed, transposed=False, plant="first"):
+    a, b, want = _exact_case(torch, path, n, k, m, seed, plant=plant)
     a, b = a[0], b[0]
+    _assert_datapath(path, a, b)
     if transposed:
         a = np.ascontiguousarray(a.T)
     da, db = _dev(torch, path, a), _dev(torch, path, b)
@@ -255,17 +265,18 @@ def test_multiwave_exact_dmma(torch, mm, tile_rows):
 def test_edge_shapes_exact(torch, mm, ctx, path, edge):
     w = WIDTH[path]
     n, k, m = (1, w, w) if edge == "1xWxW" else (129, 3 * w, 17 * w)
-    _exact_call(torch, mm, ctx, path, n, k, m, seed=23)
+    _exact_call(torch, mm, ctx, path, n, k, m, seed=23, plant="last")
     if path != "dmma":   # DMMA takes a transposed A only for even N
-        _exact_call(torch, mm, ctx, path, n, k, m, seed=23, transposed=True)
+        _exact_call(torch, mm, ctx, path, n, k, m, seed=23, transposed=True, plant="last")
 
 
-@pytest.mark.parametrize("route", ["a", "at", "b"])
-def test_tf32_ties_round_away_from_zero(torch, mm, ctx, route):
-    """Odd 12-bit integers are TF32 ties: the exact product of rna-rounded operands pins the rounding mode on the
-    row-major A, transposed A and B routes."""
+def _tie_call(torch, mm, ctx, route, path):
+    """The tie data of `route` on the datapath that `path` names, against the exact product of the rounded operands."""
     n, k, m = 129, 64, 272
     a, b = tn.tie_operands("b" if route == "b" else "a", n, k, m, seed=24)
+    if path == "tf32":
+        a[n - 1] *= np.float32(tn.PLANT_SCALE)
+    _assert_datapath(path, a, b)
     want = tn.store("tf32", tn.rna_tf32(a).astype(np.float64) @ tn.rna_tf32(b).astype(np.float64))
     flags = 0
     if route == "at":
@@ -274,21 +285,38 @@ def test_tf32_ties_round_away_from_zero(torch, mm, ctx, route):
     tn.check_exact("tf32", got, want)
 
 
+@pytest.mark.parametrize("route", ["a", "at", "b"])
+def test_tf32_ties_round_away_from_zero(torch, mm, ctx, route):
+    """Odd 12-bit integers are TF32 ties: the exact product of rna-rounded operands pins the rounding mode on the
+    row-major A, transposed A and B routes.  The rounded ties are halves, so the call runs on the f16 datapath."""
+    _tie_call(torch, mm, ctx, route, "tf32h")
+
+
+@pytest.mark.parametrize("route", ["a", "at", "b"])
+def test_tf32_ties_round_away_from_zero_on_the_tf32_datapath(torch, mm, ctx, route):
+    """The same ties with A's last row times 2^20 (still exact): no half holds it, so the call runs on TF32."""
+    _tie_call(torch, mm, ctx, route, "tf32")
+
+
 # ---- c. batched, multi-wave, exact ----------------------------------------------------------------------------
 
-BATCHED = {"tf32": (513, 272, 1040), "f16": (513, 288, 1088), "u8": (513, 320, 1088), "dmma": (513, 272, 1040)}
+BATCHED = {"tf32": (513, 272, 1040), "tf32h": (513, 272, 1040), "f16": (513, 288, 1088), "u8": (513, 320, 1088),
+           "dmma": (513, 272, 1040)}
 
 
 @pytest.mark.parametrize("shared", ["none", "a", "b"])
 @pytest.mark.parametrize("path", sorted(BATCHED))
 def test_batched_multiwave_exact(torch, mm, ctx, path, shared):
     """Batch 9: 15 tiles per problem, 135 on 66 CTA groups (the DMMA kernel is not persistent: per-problem offsets).
-    Each problem carries its own power-of-two scale and is compared with its own exact product."""
+    Each problem carries its own power-of-two scale and is compared with its own exact product.  "tf32": every copy
+    of A has its row times 2^20, first and last rows alternating, the last problem's at its last row."""
     n, k, m = BATCHED[path]
     batch = 9
     sa, sb = shared == "a", shared == "b"
     a, b, want = _exact_case(torch, path, n, k, m, 25, batch, sa, sb)
     flags = (mm.FLAG_BATCH_SHARED_A if sa else 0) | (mm.FLAG_BATCH_SHARED_B if sb else 0)
+    for i in range(batch):
+        _assert_datapath(path, a[0 if sa else i], b[0 if sb else i])
     da, db = _dev(torch, path, a), _dev(torch, path, b)
     for poison in _poisons(path):
         got = _run(torch, mm, ctx, path, da, db, n, k, m, flags=flags, batch=batch, poison=poison)
