@@ -445,9 +445,19 @@ struct Pipeline {
     mm::HalfScratch hs;
     if (path == kPathTcgen05) {
       hs = mm::tcgen05_half_scratch(ctx->scratch.ptr, ctx->scratch.bytes, dtype, rows, k, m, flags, t);
-      if (hs.fits_b) MM_CUDA_TRY(cudaMemsetAsync(hs.fits_b, 1, hs.flag_bytes, ctx->stream));
-      rc = mm::tcgen05_prepare_b_async(dtype, src, db, ctx->scratch.ptr, ctx->scratch.bytes, k, m, flags, t, ctx->stream,
-                                       ctx->side, ctx->ev_fork, ctx->ev_join, &pb, 1, hs.b, hs.fits_b);
+      if (hs.fits_b) {
+        // float: the one-pass preparation of B from this GPU's whole B (the peers' slices gathered in first)
+        MM_CUDA_TRY(cudaMemsetAsync(hs.fits_b, 1, hs.flag_bytes, ctx->stream));
+        if (bp.parts_dev != nullptr) rc = mm::gather_b_rows(src, db, es, k, m, ctx->stream);
+        if (rc == MM_OK) {
+          rc = mm::tcgen05_prepare_float(false, nullptr, 0, 0, db, rows, k, m, flags, t, mm::GemmBatch{},
+                                         ctx->scratch.ptr, ctx->scratch.bytes, ctx->stream);
+        }
+        pb.b_op = ctx->scratch.ptr;
+      } else {
+        rc = mm::tcgen05_prepare_b_async(dtype, src, db, ctx->scratch.ptr, ctx->scratch.bytes, k, m, flags, t,
+                                         ctx->stream, ctx->side, ctx->ev_fork, ctx->ev_join, &pb, 1);
+      }
       if (rc != MM_OK) return rc;
       aprep = static_cast<unsigned char *>(ctx->scratch.ptr) + mm::tcgen05_bt_bytes(dtype, k, m, flags, t);
     } else if (bp.parts_dev != nullptr) {
@@ -455,17 +465,23 @@ struct Pipeline {
       if (rc != MM_OK) return rc;
     }
     // With fp16 copies every chunk's preparation clears the one fits flag of A, and the GEMMs start once all of A is
-    // prepared: each chunk then takes the datapath of the whole A, so the chunks' C is the single call's, bit for bit.
+    // prepared and the TF32 copies still owed are written: each chunk then takes the datapath of the whole A, so the
+    // chunks' C is the single call's, bit for bit.
     const bool prepare_first = hs.fits_a != nullptr;
     std::vector<const void *> a_ops(chunks);
     auto prepare = [&](unsigned i) -> int {
       const size_t r0 = size_t(i) * chunk_rows, nr = std::min<size_t>(chunk_rows, rows - r0);
       MM_CUDA_TRY(cudaStreamWaitEvent(ctx->stream, ev_a(i), 0));
       if (path != kPathTcgen05) return MM_OK;
+      if (hs.fits_a != nullptr) {
+        a_ops[i] = aprep + r0 * k * es;
+        return mm::tcgen05_prepare_float(false, da + (ta ? 0 : r0 * k * es), unsigned(r0), unsigned(nr), nullptr, rows,
+                                         k, m, flags, t, mm::GemmBatch{}, ctx->scratch.ptr, ctx->scratch.bytes,
+                                         ctx->stream);
+      }
       const size_t a_scale = (dtype == MM_DTYPE_FLOAT && (flags & MM_FLAG_TF32X3)) ? 3 : 1;
       return mm::tcgen05_prepare_a(dtype, da + (ta ? 0 : r0 * k * es), aprep + (ta ? 0 : r0 * k * es * a_scale),
-                                   unsigned(nr), k, flags, t, &a_ops[i], ctx->stream, 1,
-                                   hs.a ? static_cast<unsigned char *>(hs.a) + r0 * k * 2 : nullptr, hs.fits_a);
+                                   unsigned(nr), k, flags, t, &a_ops[i], ctx->stream, 1);
     };
     auto compute = [&](unsigned i) -> int {
       const size_t r0 = size_t(i) * chunk_rows, nr = std::min<size_t>(chunk_rows, rows - r0);
@@ -489,6 +505,10 @@ struct Pipeline {
       for (unsigned i = 0; i < chunks && rc == MM_OK; ++i) rc = prepare(i);
     }
     if (rc == MM_OK && agree != nullptr) rc = (*agree)(hs.fits_a, ctx->stream);
+    if (rc == MM_OK && prepare_first) {  // one second pass over B and all of A
+      rc = mm::tcgen05_prepare_float(true, da, 0, rows, db, rows, k, m, flags, t, mm::GemmBatch{}, ctx->scratch.ptr,
+                                     ctx->scratch.bytes, ctx->stream);
+    }
     for (unsigned i = 0; i < chunks && rc == MM_OK; ++i) {
       if (!prepare_first) rc = prepare(i);
       if (rc == MM_OK) rc = compute(i);

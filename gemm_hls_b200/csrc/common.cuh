@@ -123,13 +123,16 @@ struct HalfOperands {
   const void *a = nullptr, *b = nullptr;
   const unsigned int *fits_a = nullptr, *fits_b = nullptr;
 };
-// Where the preparation writes them.  fits: [one word per B copy][one word per A copy] just before the counters at the
-// scratch's end, set nonzero (cudaMemsetAsync of flag_bytes) before the preparation, cleared by any preparation block
-// that meets a value which is not exactly a normal half or zero (fits_half.h).  All null when the call stays on TF32:
-// not float, MM_FLAG_TF32X3 (its lo parts are far below half range) or the tf32_no_round experiment (raw float bits).
+// Where the preparation writes them.  Just before the counters at the scratch's end: [one fits word per B copy][one per
+// A copy][pending map of B][pending map of A], all set nonzero by one cudaMemsetAsync of flag_bytes before the
+// preparation.  A fits word is cleared by any preparation item that meets a value which is not exactly a normal half or
+// zero (fits_half.h).  The pending maps hold one byte per 64 x 64 item of each copy: 1 while the item's TF32 copy is
+// owed (tcgen05_prepare_float).  All null when the call stays on TF32: not float, MM_FLAG_TF32X3 (its lo parts are far
+// below half range) or the tf32_no_round experiment (raw float bits).
 struct HalfScratch {
   void *a = nullptr, *b = nullptr;
   unsigned int *fits_a = nullptr, *fits_b = nullptr;
+  unsigned char *pending_a = nullptr, *pending_b = nullptr;
   size_t flag_bytes = 0;
   HalfOperands operands() const { return HalfOperands{a, b, fits_a, fits_b}; }
 };
@@ -162,11 +165,10 @@ Tcgen05Counters tcgen05_counters(void *scratch, size_t scratch_bytes);
 // a time, in the order the GEMM's rasterisation consumes them) as a co-resident persistent kernel and
 // publishes each panel through ready[panel]; *ready_target receives the count that means "complete".
 // `copies` packed K x M problems of B are prepared into `copies` packed M x K copies (K-major path only).
-// `bt16` / `fits` non-null (HalfScratch): float's K-major copy is also written as halves into `bt16`, and fits[i]
-// cleared when copy i has a value that is not a half.
+// Not for float on the default datapath: see tcgen05_prepare_float.
 int tcgen05_prepare_b(int dtype, const BSource &src, void *bt, unsigned k, unsigned m, int flags, const Tuning &t,
                       const void **b_op, unsigned int *ready, unsigned *ready_target, cudaStream_t stream,
-                      unsigned copies = 1, void *bt16 = nullptr, unsigned int *fits = nullptr);
+                      unsigned copies = 1);
 // Fork / join wrapper around tcgen05_prepare_b for the launchers: decides whether the preparation
 // overlaps the GEMM (float rounding, or any gather of peer slices, with the MN-major B path and a side
 // stream), zeroes the panel counters in stream order, runs the pass on `side` — ENQUEUED BEFORE the
@@ -181,12 +183,19 @@ struct PreparedB {
 };
 int tcgen05_prepare_b_async(int dtype, const BSource &src, void *local_b, void *scratch, size_t scratch_bytes,
                             unsigned k, unsigned m, int flags, const Tuning &t, cudaStream_t stream, cudaStream_t side,
-                            cudaEvent_t ev_fork, cudaEvent_t ev_join, PreparedB *out, unsigned copies = 1,
-                            void *bt16 = nullptr, unsigned int *fits = nullptr);
-// `copies` packed problems of `rows` rows each.  `aprep16` / `fits` as for tcgen05_prepare_b: problem i clears fits[i].
+                            cudaEvent_t ev_fork, cudaEvent_t ev_join, PreparedB *out, unsigned copies = 1);
+// `copies` packed problems of `rows` rows each.  Not for float on the default datapath: see tcgen05_prepare_float.
 int tcgen05_prepare_a(int dtype, const void *a, void *aprep, unsigned rows, unsigned k, int flags, const Tuning &t,
-                      const void **a_op, cudaStream_t stream, unsigned copies = 1, void *aprep16 = nullptr,
-                      unsigned int *fits = nullptr);
+                      const void **a_op, cudaStream_t stream, unsigned copies = 1);
+// Float on the default datapath (HalfScratch non-empty): both operands into the scratch's copies, the TF32 copy (B^T
+// at the scratch's start, A at tcgen05_bt_bytes) or the fp16 copy of each 64 x 64 item, whichever the GEMM will read.
+// Needs the memset of HalfScratch::flag_bytes first.  complete = false: the first pass over B (`b` non-null, one K x M
+// array per copy) and rows [row0, row0 + rows) of A (`a` non-null, pointing at row row0; row0 % 64 == 0; A stored
+// K x N only whole); it may run per chunk of A.  complete = true, once the fits words are final (after any multi-GPU
+// agreement): the second pass over the whole of both, which writes the TF32 copies still owed.  One launch each.
+int tcgen05_prepare_float(bool complete, const void *a, unsigned row0, unsigned rows, const void *b, unsigned n,
+                          unsigned k, unsigned m, int flags, const Tuning &t, const GemmBatch &batch, void *scratch,
+                          size_t scratch_bytes, cudaStream_t stream);
 // `tile_sync`: device counter for the kernel's soft wave barrier, or null.  `b_ready` non-null: the
 // producer waits for b_ready[column tile] >= b_ready_target before it fetches a tile's B panel.
 int tcgen05_gemm(int dtype, const void *a_op, const void *b_op, void *c, unsigned rows, unsigned k, unsigned m,

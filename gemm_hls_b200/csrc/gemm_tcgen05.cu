@@ -70,16 +70,12 @@ __device__ __forceinline__ uint32_t half2_bits(float lo, float hi) {
   return *reinterpret_cast<const uint32_t *>(&h);
 }
 
-// dst[i] = rna_tf32(src[i]); count4 float4 per problem, blockIdx.y = problem of a batch (packed).  HALF: dst16 gets the
-// same values as halves, and fits[problem] is cleared when one of them is not exactly a half (one store per block).
-template <bool HALF>
+// dst[i] = rna_tf32(src[i]); count4 float4 per problem, blockIdx.y = problem of a batch (packed).
 __global__ void __launch_bounds__(256)
-round_tf32_kernel(const float4 *__restrict__ src, float4 *__restrict__ dst, size_t count4, uint2 *__restrict__ dst16,
-                  unsigned int *__restrict__ fits) {
+round_tf32_kernel(const float4 *__restrict__ src, float4 *__restrict__ dst, size_t count4) {
   src += size_t(blockIdx.y) * count4;
   dst += size_t(blockIdx.y) * count4;
   const size_t stride = size_t(gridDim.x) * blockDim.x;
-  bool fit = true;
   for (size_t i = size_t(blockIdx.x) * blockDim.x + threadIdx.x; i < count4; i += stride) {
     float4 v = src[i];
     v.x = round_tf32(v.x);
@@ -87,14 +83,230 @@ round_tf32_kernel(const float4 *__restrict__ src, float4 *__restrict__ dst, size
     v.z = round_tf32(v.z);
     v.w = round_tf32(v.w);
     dst[i] = v;
-    if constexpr (HALF) {
-      dst16[size_t(blockIdx.y) * count4 + i] = make_uint2(half2_bits(v.x, v.y), half2_bits(v.z, v.w));
-      fit = fit && tf32_fits_half(__float_as_uint(v.x)) && tf32_fits_half(__float_as_uint(v.y)) &&
-            tf32_fits_half(__float_as_uint(v.z)) && tf32_fits_half(__float_as_uint(v.w));
+  }
+}
+
+// ---- float on the default datapath: one preparation pass that writes the copy the GEMM will read ---------------
+// A problem reads either the TF32 copies of its operands or the fp16 copies, never both (HalfOperands).  So the first
+// pass, prep_float_operands_kernel, writes one copy per item: an item is one 64 x 64 tile of a source operand, and it
+// is prepared in one of two modes, read once from the fits words at its start and uniform across the block:
+//   optimistic   round to TF32, write the fp16 copy only, and clear the copy's fits word when a value does not fit;
+//                the item's TF32 copy stays owed (its byte in the pending map stays 1).
+//   settled      a fits word that already reads 0 proves that every problem reading this copy runs on TF32 (its own
+//                word, or the partner operand's word when this copy is read by one problem only); write the TF32 copy
+//                only and clear the item's pending byte.
+// Within a call the words only go from nonzero to zero (the memset, these passes, the multi-GPU agreement), so a
+// settled item is never needed as fp16.  The second pass, complete_tf32_kernel, runs once the words are final (after
+// the multi-GPU agreement): for each copy that some problem reads on TF32 it writes the TF32 copy of every item still
+// owed, reading the source again.  Data that fits costs 6 bytes per element (read fp32, write fp16), data found not to
+// fit early 8 (read, write TF32).
+constexpr int FP_TILE = 64;
+constexpr int FP_THREADS = 256;
+
+struct FloatPrepOperand {
+  const float *src = nullptr;  // `copies` packed src_rows x src_cols row-major sources
+  float *dst = nullptr;        // TF32 copies, K-major: the source itself (flat) or its transpose
+  __half *dst16 = nullptr;     // fp16 copies, same layout
+  unsigned int *fits = nullptr;            // one word per copy
+  const unsigned int *partner = nullptr;   // the other operand's words; null when a copy is read by several problems
+  uint32_t partner_stride = 0;             // 1: copy i's problem reads the other operand's copy i; 0: its only copy
+  const unsigned int *other = nullptr;     // all of the other operand's words (other_count), for a shared copy
+  uint32_t other_count = 0;
+  unsigned char *pending = nullptr;        // one byte per item: 1 = its TF32 copy is still owed
+  uint32_t src_rows = 0, src_cols = 0, tiles_c = 0, items_per_copy = 0, items = 0;
+  bool transpose = false;  // dst = the transpose of src (B, or A stored K x N)
+  bool vec = false;        // src rows are whole float4 (src_cols % 4 == 0)
+};
+struct FloatPrepArgs {
+  FloatPrepOperand op[2];
+};
+
+struct FloatItemSmem {
+  float tile[FP_TILE][FP_TILE + 1];
+  int settled;
+};
+
+// Whether copy `copy` of `o` is certainly read on TF32 by every problem that reads it, from the words as they are now.
+__device__ __forceinline__ bool settled_now(const FloatPrepOperand &o, uint32_t copy) {
+  const volatile unsigned int *own = o.fits;
+  if (own[copy] == 0u) return true;
+  const volatile unsigned int *partner = o.partner;
+  return partner != nullptr && partner[copy * o.partner_stride] == 0u;
+}
+
+// One item.  COMPLETE (complete_tf32_kernel): the TF32 copy only, nothing else touched.  Otherwise the mode is read
+// from the words, and the item's pending byte or the copy's fits word updated at its end.  Ends with a barrier.
+template <bool COMPLETE>
+__device__ __forceinline__ void float_item(const FloatPrepOperand &o, uint32_t item, FloatItemSmem &sm) {
+  const uint32_t t = threadIdx.x;
+  const uint32_t copy = item / o.items_per_copy;
+  const uint32_t tile_i = item - copy * o.items_per_copy;
+  const uint32_t r0 = tile_i / o.tiles_c * FP_TILE, c0 = tile_i % o.tiles_c * FP_TILE;
+  const size_t base = size_t(copy) * o.src_rows * o.src_cols;
+  const float *src = o.src + base;
+  float v[16];
+  bool fit = true;
+  // loads: flat items as 8-float groups (row q / 8, columns 8 * (q % 8)), transposed items as float4 (row f / 16,
+  // columns 4 * (f % 16)); both read whole 256-byte row segments per 16 (8) lanes
+  if (!o.transpose) {
+#pragma unroll
+    for (int j = 0; j < 2; ++j) {
+      const uint32_t q = t + FP_THREADS * j, r = r0 + q / 8, c = c0 + 8 * (q % 8);
+      float4 x = make_float4(0.f, 0.f, 0.f, 0.f), y = x;
+      if (r < o.src_rows && c < o.src_cols) {
+        const float4 *p = reinterpret_cast<const float4 *>(src + size_t(r) * o.src_cols + c);
+        x = p[0];
+        y = p[1];
+      }
+      v[8 * j + 0] = x.x; v[8 * j + 1] = x.y; v[8 * j + 2] = x.z; v[8 * j + 3] = x.w;
+      v[8 * j + 4] = y.x; v[8 * j + 5] = y.y; v[8 * j + 6] = y.z; v[8 * j + 7] = y.w;
+    }
+  } else {
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const uint32_t f = t + FP_THREADS * j, r = r0 + f / 16, c = c0 + 4 * (f % 16);
+      float4 x = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (r < o.src_rows) {
+        const float *p = src + size_t(r) * o.src_cols + c;
+        if (o.vec) {
+          if (c < o.src_cols) x = *reinterpret_cast<const float4 *>(p);
+        } else {
+          if (c + 0 < o.src_cols) x.x = p[0];
+          if (c + 1 < o.src_cols) x.y = p[1];
+          if (c + 2 < o.src_cols) x.z = p[2];
+          if (c + 3 < o.src_cols) x.w = p[3];
+        }
+      }
+      v[4 * j + 0] = x.x; v[4 * j + 1] = x.y; v[4 * j + 2] = x.z; v[4 * j + 3] = x.w;
     }
   }
-  if constexpr (HALF) {
-    if (__syncthreads_or(!fit) && threadIdx.x == 0) fits[blockIdx.y] = 0u;
+#pragma unroll
+  for (int e = 0; e < 16; ++e) {
+    v[e] = round_tf32(v[e]);
+    if (!COMPLETE) fit = fit && tf32_fits_half(__float_as_uint(v[e]));  // padding is 0, which fits
+  }
+  if (o.transpose) {
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const uint32_t f = t + FP_THREADS * j, r = f / 16, c = 4 * (f % 16);
+#pragma unroll
+      for (int e = 0; e < 4; ++e) sm.tile[r][c + e] = v[4 * j + e];
+    }
+  }
+  if (!COMPLETE && t == 0) sm.settled = settled_now(o, copy);
+  __syncthreads();
+  const bool settled = COMPLETE || sm.settled;
+  float *dst = o.dst + base;
+  __half *dst16 = o.dst16 + base;
+  const uint32_t ld = o.transpose ? o.src_rows : o.src_cols;  // destination row length (K)
+  if (!o.transpose) {
+#pragma unroll
+    for (int j = 0; j < 2; ++j) {
+      const uint32_t q = t + FP_THREADS * j, r = r0 + q / 8, c = c0 + 8 * (q % 8);
+      if (r >= o.src_rows || c >= o.src_cols) continue;
+      const size_t off = size_t(r) * ld + c;
+      const float *w = v + 8 * j;
+      if (settled) {
+        reinterpret_cast<float4 *>(dst + off)[0] = make_float4(w[0], w[1], w[2], w[3]);
+        reinterpret_cast<float4 *>(dst + off)[1] = make_float4(w[4], w[5], w[6], w[7]);
+      } else {
+        *reinterpret_cast<uint4 *>(dst16 + off) =
+            make_uint4(half2_bits(w[0], w[1]), half2_bits(w[2], w[3]), half2_bits(w[4], w[5]), half2_bits(w[6], w[7]));
+      }
+    }
+  } else if (settled) {
+    // 4 k-values of destination row m per 16-byte store; a warp covers 4 rows x 32 k: conflict-free column reads
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const uint32_t idx = t + FP_THREADS * j, m = idx % 4 + 4 * (idx / 64), g = idx / 4 % 16;
+      if (c0 + m >= o.src_cols || r0 + 4 * g >= o.src_rows) continue;
+      float4 x;
+      x.x = sm.tile[4 * g + 0][m];
+      x.y = sm.tile[4 * g + 1][m];
+      x.z = sm.tile[4 * g + 2][m];
+      x.w = sm.tile[4 * g + 3][m];
+      *reinterpret_cast<float4 *>(dst + size_t(c0 + m) * ld + r0 + 4 * g) = x;
+    }
+  } else {
+    // 8 k-values per 16-byte store of halves; a warp covers 8 rows x 32 k
+#pragma unroll
+    for (int j = 0; j < 2; ++j) {
+      const uint32_t idx = t + FP_THREADS * j, m = idx % 8 + 8 * (idx / 64), g = idx / 8 % 8;
+      if (c0 + m >= o.src_cols || r0 + 8 * g >= o.src_rows) continue;
+      float x[8];
+#pragma unroll
+      for (int e = 0; e < 8; ++e) x[e] = sm.tile[8 * g + e][m];
+      *reinterpret_cast<uint4 *>(dst16 + size_t(c0 + m) * ld + r0 + 8 * g) =
+          make_uint4(half2_bits(x[0], x[1]), half2_bits(x[2], x[3]), half2_bits(x[4], x[5]), half2_bits(x[6], x[7]));
+    }
+  }
+  // the barrier also frees sm for the next item
+  const int misfit = __syncthreads_or(!settled && !fit);
+  if (!COMPLETE && t == 0) {
+    if (settled) o.pending[item] = 0;
+    else if (misfit) o.fits[copy] = 0u;
+  }
+}
+
+// First pass: every item of both operands, dealt round-robin to a persistent grid (op[0]'s items first).
+__global__ void __launch_bounds__(FP_THREADS)
+prep_float_operands_kernel(const FloatPrepArgs args) {
+  __shared__ FloatItemSmem sm;
+  const uint32_t items0 = args.op[0].items, total = items0 + args.op[1].items;
+  for (uint32_t item = blockIdx.x; item < total; item += gridDim.x) {
+    if (item < items0) float_item<false>(args.op[0], item, sm);
+    else float_item<false>(args.op[1], item - items0, sm);
+  }
+}
+
+// Whether some problem reading copy `copy` of `o` runs on TF32, from the final words.  `any_other_zero`: one of the
+// other operand's words is 0 (what decides for a copy that several problems read).
+__device__ __forceinline__ bool read_on_tf32(const FloatPrepOperand &o, uint32_t copy, bool any_other_zero) {
+  if (o.fits[copy] == 0u) return true;
+  return o.partner != nullptr ? o.partner[copy * o.partner_stride] == 0u : any_other_zero;
+}
+
+// Second pass: the TF32 copy of every item still owed whose copy some problem reads on TF32.  Each block gathers up
+// to 256 of its items per round with one load per thread, so that a call that owes nothing costs one round.
+__global__ void __launch_bounds__(FP_THREADS)
+complete_tf32_kernel(const FloatPrepArgs args) {
+  __shared__ FloatItemSmem sm;
+  __shared__ uint32_t owed[FP_THREADS];
+  __shared__ uint32_t owed_count;
+  const uint32_t t = threadIdx.x;
+  // any_zero(o): one of the other operand's words is 0; only a copy that several problems read asks
+  auto any_zero = [t](const FloatPrepOperand &o) {
+    bool z = false;
+    if (o.items != 0 && o.partner == nullptr) {
+      for (uint32_t w = t; w < o.other_count; w += FP_THREADS) z = z || o.other[w] == 0u;
+    }
+    return __syncthreads_or(z) != 0;
+  };
+  const bool zero0 = any_zero(args.op[0]), zero1 = any_zero(args.op[1]);
+  const uint32_t items0 = args.op[0].items, total = items0 + args.op[1].items;
+  if (t == 0) owed_count = 0;
+  __syncthreads();
+  for (size_t first = blockIdx.x; first < total; first += size_t(FP_THREADS) * gridDim.x) {
+    const size_t slot = first + size_t(t) * gridDim.x;
+    if (slot < total) {
+      const uint32_t item = uint32_t(slot);
+      const bool second = item >= items0;
+      const FloatPrepOperand &o = second ? args.op[1] : args.op[0];
+      const uint32_t local = second ? item - items0 : item;
+      if (read_on_tf32(o, local / o.items_per_copy, second ? zero1 : zero0) && o.pending[local] != 0) {
+        owed[atomicAdd(&owed_count, 1u)] = item;
+      }
+    }
+    __syncthreads();
+    const uint32_t count = owed_count;
+    for (uint32_t j = 0; j < count; ++j) {
+      const uint32_t it = owed[j];
+      if (it < items0) float_item<true>(args.op[0], it, sm);
+      else float_item<true>(args.op[1], it - items0, sm);
+    }
+    __syncthreads();
+    if (t == 0) owed_count = 0;
+    __syncthreads();
   }
 }
 
@@ -169,23 +381,12 @@ prep_b_panels_kernel(const uint4 *__restrict__ single, const uint4 *const *__res
   }
 }
 
-template <typename T, bool ROUND>
-__device__ __forceinline__ T prep_value(T x) {
-  return x;
-}
-template <>
-__device__ __forceinline__ float prep_value<float, true>(float x) {
-  return round_tf32(x);
-}
-
-// dst[c][r] = f(src[r][c]) for src of shape src_rows x src_cols (row-major): 64 x 64 tiles through
+// dst[c][r] = src[r][c] for src of shape src_rows x src_cols (row-major): 64 x 64 tiles through
 // shared memory so that both the reads and the writes are row-contiguous.  blockIdx.z = problem of a
-// batch: packed sources, packed destinations.  ROUND (float to TF32): dst16 gets the rounded values as halves too, and
-// fits[problem] is cleared when one of them is not exactly a half, as in round_tf32_kernel.
-template <typename T, bool ROUND>
+// batch: packed sources, packed destinations.
+template <typename T>
 __global__ void __launch_bounds__(256)
-transpose_prep_kernel(const T *__restrict__ src, T *__restrict__ dst, uint32_t src_rows,
-                      uint32_t src_cols, __half *__restrict__ dst16, unsigned int *__restrict__ fits) {
+transpose_prep_kernel(const T *__restrict__ src, T *__restrict__ dst, uint32_t src_rows, uint32_t src_cols) {
   constexpr int TILE = 64;
   constexpr int PAD = (sizeof(T) >= 4) ? 1 : 2;
   __shared__ T tile[TILE][TILE + PAD];
@@ -198,24 +399,13 @@ transpose_prep_kernel(const T *__restrict__ src, T *__restrict__ dst, uint32_t s
 #pragma unroll 4
   for (int i = y; i < TILE; i += 4) {
     const uint32_t r = r0 + i, c = c0 + x;
-    if (r < src_rows && c < src_cols) tile[i][x] = prep_value<T, ROUND>(src[size_t(r) * src_cols + c]);
+    if (r < src_rows && c < src_cols) tile[i][x] = src[size_t(r) * src_cols + c];
   }
   __syncthreads();
-  bool fit = true;
 #pragma unroll 4
   for (int i = y; i < TILE; i += 4) {
     const uint32_t c = c0 + i, r = r0 + x;  // dst row = src col
-    if (c < src_cols && r < src_rows) {
-      const T v = tile[x][i];
-      dst[size_t(c) * src_rows + r] = v;
-      if constexpr (ROUND) {
-        dst16[size_t(blockIdx.z) * src_rows * src_cols + size_t(c) * src_rows + r] = __float2half_rn(v);
-        fit = fit && tf32_fits_half(__float_as_uint(v));
-      }
-    }
-  }
-  if constexpr (ROUND) {
-    if (__syncthreads_or(!fit) && threadIdx.x == 0) fits[blockIdx.z] = 0u;
+    if (c < src_cols && r < src_rows) dst[size_t(c) * src_rows + r] = tile[x][i];
   }
 }
 
@@ -302,31 +492,22 @@ split3_transpose_kernel(const float *__restrict__ src, float *__restrict__ dst, 
 
 size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
-template <typename T, bool ROUND>
+template <typename T>
 void launch_transpose(const void *src, void *dst, uint32_t src_rows, uint32_t src_cols, cudaStream_t stream,
-                      unsigned copies, void *dst16 = nullptr, unsigned int *fits = nullptr) {
+                      unsigned copies) {
   dim3 grid((src_cols + 63) / 64, (src_rows + 63) / 64, copies);
-  transpose_prep_kernel<T, ROUND><<<grid, 256, 0, stream>>>(static_cast<const T *>(src), static_cast<T *>(dst),
-                                                           src_rows, src_cols, static_cast<__half *>(dst16), fits);
+  transpose_prep_kernel<T><<<grid, 256, 0, stream>>>(static_cast<const T *>(src), static_cast<T *>(dst), src_rows,
+                                                     src_cols);
 }
 
-// Rounds `copies` packed problems of count4 float4 each; with `dst16` the fp16 copies and fits flags too.
-int launch_round(const void *src, void *dst, size_t count4, unsigned copies, void *dst16, unsigned int *fits,
-                 cudaStream_t stream) {
+// Rounds `copies` packed problems of count4 float4 each.
+int launch_round(const void *src, void *dst, size_t count4, unsigned copies, cudaStream_t stream) {
   const int blocks = int(std::min<size_t>((count4 + 255) / 256, size_t(num_sms()) * 16));
   const dim3 grid(std::max(blocks, 1), copies);
-  const float4 *s = static_cast<const float4 *>(src);
-  float4 *d = static_cast<float4 *>(dst);
-  if (dst16 != nullptr) {
-    // see tcgen05_prepare_b
-    MM_CUDA_TRY(cudaFuncSetAttribute(round_tf32_kernel<true>, cudaFuncAttributePreferredSharedMemoryCarveout,
-                                     cudaSharedmemCarveoutMaxShared));
-    round_tf32_kernel<true><<<grid, 256, 0, stream>>>(s, d, count4, static_cast<uint2 *>(dst16), fits);
-  } else {
-    MM_CUDA_TRY(cudaFuncSetAttribute(round_tf32_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout,
-                                     cudaSharedmemCarveoutMaxShared));
-    round_tf32_kernel<false><<<grid, 256, 0, stream>>>(s, d, count4, nullptr, nullptr);
-  }
+  // see tcgen05_prepare_b
+  MM_CUDA_TRY(cudaFuncSetAttribute(round_tf32_kernel, cudaFuncAttributePreferredSharedMemoryCarveout,
+                                   cudaSharedmemCarveoutMaxShared));
+  round_tf32_kernel<<<grid, 256, 0, stream>>>(static_cast<const float4 *>(src), static_cast<float4 *>(dst), count4);
   return MM_OK;
 }
 
@@ -382,8 +563,13 @@ size_t a_copy_bytes(int dtype, unsigned n, unsigned k, int flags, unsigned a_cop
   if (dtype != MM_DTYPE_FLOAT && !(flags & MM_FLAG_TRANSPOSED_A)) return 0;
   return align_up(size_t(a_copies) * n * k * elem_bytes(dtype) * (split3(dtype, flags) ? 3 : 1), 1024);
 }
-size_t fits_bytes(const GemmBatch &batch) {
-  return align_up(size_t(batch.a_copies() + batch.b_copies()) * sizeof(unsigned int), 1024);
+// 64 x 64 items of one copy of a rows x cols operand (either orientation: the count is the same)
+uint32_t float_items(unsigned rows, unsigned cols) { return ceil_div(rows, FP_TILE) * ceil_div(cols, FP_TILE); }
+// [fits words of B][fits words of A][pending map of B][pending map of A]
+size_t fits_bytes(unsigned n, unsigned k, unsigned m, const GemmBatch &batch) {
+  return align_up(size_t(batch.a_copies() + batch.b_copies()) * sizeof(unsigned int) +
+                      size_t(batch.b_copies()) * float_items(k, m) + size_t(batch.a_copies()) * float_items(n, k),
+                  1024);
 }
 
 size_t tcgen05_bt_bytes(int dtype, unsigned k, unsigned m, int flags, const Tuning &t, unsigned b_copies) {
@@ -396,7 +582,7 @@ size_t tcgen05_scratch_bytes(int dtype, unsigned n, unsigned k, unsigned m, int 
                              const GemmBatch &batch) {
   size_t bytes = TAIL_BYTES + tcgen05_bt_bytes(dtype, k, m, flags, t, batch.b_copies());  // counters (tail) + B copies
   bytes += a_copy_bytes(dtype, n, k, flags, batch.a_copies());
-  if (half_copies(dtype, flags, t)) bytes += align_up(size_t(batch.a_copies()) * n * k * 2, 1024) + fits_bytes(batch);
+  if (half_copies(dtype, flags, t)) bytes += align_up(size_t(batch.a_copies()) * n * k * 2, 1024) + fits_bytes(n, k, m, batch);
   return bytes;
 }
 
@@ -408,9 +594,11 @@ HalfScratch tcgen05_half_scratch(void *scratch, size_t scratch_bytes, int dtype,
   const size_t bt = tcgen05_bt_bytes(dtype, k, m, flags, t, batch.b_copies());
   h.b = sp + b_copy_bytes(dtype, k, m, flags, batch.b_copies());
   h.a = sp + bt + a_copy_bytes(dtype, n, k, flags, batch.a_copies());
-  h.flag_bytes = fits_bytes(batch);
+  h.flag_bytes = fits_bytes(n, k, m, batch);
   h.fits_b = reinterpret_cast<unsigned int *>(sp + scratch_bytes - TAIL_BYTES - h.flag_bytes);
   h.fits_a = h.fits_b + batch.b_copies();
+  h.pending_b = reinterpret_cast<unsigned char *>(h.fits_a + batch.a_copies());
+  h.pending_a = h.pending_b + size_t(batch.b_copies()) * float_items(k, m);
   return h;
 }
 
@@ -423,7 +611,7 @@ int gather_b_rows(const BSource &src, void *dst, size_t elem_bytes, unsigned k, 
 
 int tcgen05_prepare_b(int dtype, const BSource &src, void *bt, unsigned k, unsigned m, int flags, const Tuning &t,
                       const void **b_op, unsigned int *ready, unsigned *ready_target, cudaStream_t stream,
-                      unsigned copies, void *bt16, unsigned int *fits) {
+                      unsigned copies) {
   *b_op = bt;
   if (ready_target) *ready_target = 0;
   const bool parts = src.src != nullptr;
@@ -439,7 +627,7 @@ int tcgen05_prepare_b(int dtype, const BSource &src, void *bt, unsigned k, unsig
     if (!in_place && !parts && ready == nullptr) {
       // one local array, nobody waiting on panels: the flat elementwise pass (6.3 TB/s against the panel
       // kernel's 5.1 on a 512 MiB block — the panel order costs row-segment locality)
-      const int rc = launch_round(src.b, bt, size_t(k) * m / 4, 1, nullptr, nullptr, stream);
+      const int rc = launch_round(src.b, bt, size_t(k) * m / 4, 1, stream);
       if (rc != MM_OK) return rc;
       MM_CUDA_TRY(cudaGetLastError());
       return MM_OK;
@@ -470,15 +658,12 @@ int tcgen05_prepare_b(int dtype, const BSource &src, void *bt, unsigned k, unsig
     dim3 grid((m + 63) / 64, (k + 63) / 64, copies);
     split3_transpose_kernel<true><<<grid, 256, 0, stream>>>(static_cast<const float *>(b), static_cast<float *>(bt), k, m);
   } else if (dtype == MM_DTYPE_FLOAT) {
-    if (t.tf32_no_round()) {
-      launch_transpose<float, false>(b, bt, k, m, stream, copies);
-    } else {
-      launch_transpose<float, true>(b, bt, k, m, stream, copies, bt16, fits);
-    }
+    if (!t.tf32_no_round()) return fail(MM_ERR_INVALID, "float's rounded operands come from tcgen05_prepare_float");
+    launch_transpose<float>(b, bt, k, m, stream, copies);
   } else if (dtype == MM_DTYPE_UINT8) {
-    launch_transpose<unsigned char, false>(b, bt, k, m, stream, copies);
+    launch_transpose<unsigned char>(b, bt, k, m, stream, copies);
   } else {
-    launch_transpose<__half, false>(b, bt, k, m, stream, copies);
+    launch_transpose<__half>(b, bt, k, m, stream, copies);
   }
   MM_CUDA_TRY(cudaGetLastError());
   return MM_OK;
@@ -489,7 +674,7 @@ int tcgen05_prepare_b(int dtype, const BSource &src, void *bt, unsigned k, unsig
 // matrices) is transposed into `aprep`.  *a_op receives the operand pointer.  `copies` packed problems:
 // the row-wise passes run over copies * rows rows, the transposes take the problem from blockIdx.z.
 int tcgen05_prepare_a(int dtype, const void *a, void *aprep, unsigned rows, unsigned k, int flags, const Tuning &t,
-                      const void **a_op, cudaStream_t stream, unsigned copies, void *aprep16, unsigned int *fits) {
+                      const void **a_op, cudaStream_t stream, unsigned copies) {
   const bool transposed = (flags & MM_FLAG_TRANSPOSED_A) != 0;
   const size_t all_rows = size_t(copies) * rows;
   *a_op = a;
@@ -506,22 +691,89 @@ int tcgen05_prepare_a(int dtype, const void *a, void *aprep, unsigned rows, unsi
     }
     *a_op = aprep;
   } else if (dtype == MM_DTYPE_FLOAT) {
+    if (!t.tf32_no_round()) return fail(MM_ERR_INVALID, "float's rounded operands come from tcgen05_prepare_float");
     if (transposed) {
-      if (t.tf32_no_round()) {
-        launch_transpose<float, false>(a, aprep, k, rows, stream, copies);
-      } else {
-        launch_transpose<float, true>(a, aprep, k, rows, stream, copies, aprep16, fits);  // A stored K x N -> N x K
-      }
-      *a_op = aprep;
-    } else if (!t.tf32_no_round()) {
-      const int rc = launch_round(a, aprep, size_t(rows) * k / 4, copies, aprep16, fits, stream);
-      if (rc != MM_OK) return rc;
+      launch_transpose<float>(a, aprep, k, rows, stream, copies);  // A stored K x N -> N x K
       *a_op = aprep;
     }
   } else if (transposed) {
-    if (dtype == MM_DTYPE_UINT8) launch_transpose<unsigned char, false>(a, aprep, k, rows, stream, copies);
-    else launch_transpose<__half, false>(a, aprep, k, rows, stream, copies);
+    if (dtype == MM_DTYPE_UINT8) launch_transpose<unsigned char>(a, aprep, k, rows, stream, copies);
+    else launch_transpose<__half>(a, aprep, k, rows, stream, copies);
     *a_op = aprep;
+  }
+  MM_CUDA_TRY(cudaGetLastError());
+  return MM_OK;
+}
+
+namespace {
+FloatPrepOperand float_operand(const void *src, float *dst, __half *dst16, unsigned src_rows, unsigned src_cols,
+                               unsigned copies, bool transpose, unsigned int *fits, unsigned char *pending) {
+  FloatPrepOperand o;
+  o.src = static_cast<const float *>(src);
+  o.dst = dst;
+  o.dst16 = dst16;
+  o.fits = fits;
+  o.pending = pending;
+  o.src_rows = src_rows;
+  o.src_cols = src_cols;
+  o.tiles_c = ceil_div(src_cols, FP_TILE);
+  o.items_per_copy = float_items(src_rows, src_cols);
+  o.items = copies * o.items_per_copy;
+  o.transpose = transpose;
+  o.vec = src_cols % 4 == 0;
+  return o;
+}
+
+// A persistent grid: as many blocks as are resident at once, at most one per item.
+int float_prep_grid(const void *kernel, uint32_t items) {
+  MM_CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout,
+                                   cudaSharedmemCarveoutMaxShared));
+  int per_sm = 0;
+  MM_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, FP_THREADS, 0));
+  return int(std::max<uint32_t>(1u, std::min<uint32_t>(items, uint32_t(std::max(per_sm, 1) * num_sms()))));
+}
+}  // namespace
+
+int tcgen05_prepare_float(bool complete, const void *a, unsigned row0, unsigned rows, const void *b, unsigned n,
+                          unsigned k, unsigned m, int flags, const Tuning &t, const GemmBatch &batch, void *scratch,
+                          size_t scratch_bytes, cudaStream_t stream) {
+  const HalfScratch hs = tcgen05_half_scratch(scratch, scratch_bytes, MM_DTYPE_FLOAT, n, k, m, flags, t, batch);
+  if (hs.fits_a == nullptr) return fail(MM_ERR_INVALID, "tcgen05_prepare_float: float on the default datapath only");
+  if (row0 % FP_TILE != 0) return fail(MM_ERR_INVALID, "tcgen05_prepare_float: A's first row must be a multiple of 64");
+  unsigned char *sp = static_cast<unsigned char *>(scratch);
+  // a copy that several problems read settles on its own word only
+  const bool shared_a = batch.count > 1 && batch.shared_a, shared_b = batch.count > 1 && batch.shared_b;
+  FloatPrepArgs args;
+  if (b != nullptr) {
+    FloatPrepOperand &o = args.op[0];
+    o = float_operand(b, reinterpret_cast<float *>(sp), static_cast<__half *>(hs.b), k, m, batch.b_copies(), true,
+                      hs.fits_b, hs.pending_b);
+    o.partner = shared_b ? nullptr : hs.fits_a;
+    o.partner_stride = shared_a ? 0 : 1;
+    o.other = hs.fits_a;
+    o.other_count = batch.a_copies();
+  }
+  if (a != nullptr) {
+    const bool transposed = (flags & MM_FLAG_TRANSPOSED_A) != 0;
+    if (transposed && (row0 != 0 || rows != n)) return fail(MM_ERR_INVALID, "A stored K x N is prepared whole");
+    const size_t first = size_t(row0) * k;  // row0's element in the N x K copies; its items start at row0 / 64
+    float *aprep = reinterpret_cast<float *>(sp + tcgen05_bt_bytes(MM_DTYPE_FLOAT, k, m, flags, t, batch.b_copies()));
+    FloatPrepOperand &o = args.op[1];
+    o = float_operand(a, aprep + first, static_cast<__half *>(hs.a) + first, transposed ? k : rows,
+                      transposed ? rows : k, batch.a_copies(), transposed, hs.fits_a,
+                      hs.pending_a + size_t(row0 / FP_TILE) * ceil_div(k, FP_TILE));
+    o.partner = shared_a ? nullptr : hs.fits_b;
+    o.partner_stride = shared_b ? 0 : 1;
+    o.other = hs.fits_b;
+    o.other_count = batch.b_copies();
+  }
+  const uint32_t items = args.op[0].items + args.op[1].items;
+  if (complete) {
+    const int grid = float_prep_grid(reinterpret_cast<const void *>(complete_tf32_kernel), items);
+    complete_tf32_kernel<<<grid, FP_THREADS, 0, stream>>>(args);
+  } else {
+    const int grid = float_prep_grid(reinterpret_cast<const void *>(prep_float_operands_kernel), items);
+    prep_float_operands_kernel<<<grid, FP_THREADS, 0, stream>>>(args);
   }
   MM_CUDA_TRY(cudaGetLastError());
   return MM_OK;
@@ -567,15 +819,13 @@ int tcgen05_gemm(int dtype, const void *a_op, const void *b_op, void *c, unsigne
 
 int tcgen05_prepare_b_async(int dtype, const BSource &src, void *local_b, void *scratch, size_t scratch_bytes,
                             unsigned k, unsigned m, int flags, const Tuning &t, cudaStream_t stream, cudaStream_t side,
-                            cudaEvent_t ev_fork, cudaEvent_t ev_join, PreparedB *out, unsigned copies, void *bt16,
-                            unsigned int *fits) {
+                            cudaEvent_t ev_fork, cudaEvent_t ev_join, PreparedB *out, unsigned copies) {
   *out = PreparedB{};
   const bool in_place = tcgen05_b_in_place(dtype, flags, t);
   const bool parts = src.src != nullptr;
   if (copies != 1) {
     if (parts) return fail(MM_ERR_UNSUPPORTED, "batched calls take B from one array");
-    return tcgen05_prepare_b(dtype, src, scratch, k, m, flags, t, &out->b_op, nullptr, nullptr, stream, copies, bt16,
-                             fits);
+    return tcgen05_prepare_b(dtype, src, scratch, k, m, flags, t, &out->b_op, nullptr, nullptr, stream, copies);
   }
   if (parts && !tcgen05_b_mn(dtype, flags, t)) {
     // K-major copy requested (tuning / 3xTF32): assemble the slices first, then transpose locally
@@ -583,7 +833,7 @@ int tcgen05_prepare_b_async(int dtype, const BSource &src, void *local_b, void *
     if (rc != MM_OK) return rc;
     BSource whole;
     whole.b = local_b;
-    return tcgen05_prepare_b(dtype, whole, scratch, k, m, flags, t, &out->b_op, nullptr, nullptr, stream, 1, bt16, fits);
+    return tcgen05_prepare_b(dtype, whole, scratch, k, m, flags, t, &out->b_op, nullptr, nullptr, stream, 1);
   }
   void *bt = in_place ? local_b : scratch;
   const Tcgen05Counters cnt = tcgen05_counters(scratch, scratch_bytes);
@@ -591,7 +841,7 @@ int tcgen05_prepare_b_async(int dtype, const BSource &src, void *local_b, void *
   // the panel kernel runs (float rounding, or a gather of slices), a second stream exists, the tuning allows it
   const bool overlap = side != nullptr && t.b_overlap() != 0 && tcgen05_b_mn(dtype, flags, t) && (!in_place || parts) &&
                        panels <= B_READY_BYTES / sizeof(unsigned int);
-  if (!overlap) return tcgen05_prepare_b(dtype, src, bt, k, m, flags, t, &out->b_op, nullptr, nullptr, stream, 1, bt16, fits);
+  if (!overlap) return tcgen05_prepare_b(dtype, src, bt, k, m, flags, t, &out->b_op, nullptr, nullptr, stream, 1);
   MM_CUDA_TRY(cudaMemsetAsync(cnt.b_ready, 0, panels * sizeof(unsigned int), stream));
   MM_CUDA_TRY(cudaEventRecord(ev_fork, stream));
   MM_CUDA_TRY(cudaStreamWaitEvent(side, ev_fork, 0));
@@ -611,13 +861,13 @@ int launch_tcgen05(int dtype, const GemmArgs &g, void *scratch, size_t scratch_b
   if (g.dry_run) {
     // force the lazily loaded kernels in (prep + the GEMM variant this tuning selects) and the driver entry point
     cudaFuncAttributes attr;
-    MM_CUDA_TRY(cudaFuncGetAttributes(&attr, round_tf32_kernel<true>));
-    MM_CUDA_TRY(cudaFuncGetAttributes(&attr, round_tf32_kernel<false>));
+    MM_CUDA_TRY(cudaFuncGetAttributes(&attr, round_tf32_kernel));
     MM_CUDA_TRY(cudaFuncGetAttributes(&attr, prep_b_panels_kernel<true>));
     MM_CUDA_TRY(cudaFuncGetAttributes(&attr, prep_b_panels_kernel<false>));
-    MM_CUDA_TRY(cudaFuncGetAttributes(&attr, transpose_prep_kernel<float, true>));
-    MM_CUDA_TRY(cudaFuncGetAttributes(&attr, transpose_prep_kernel<__half, false>));
-    MM_CUDA_TRY(cudaFuncGetAttributes(&attr, transpose_prep_kernel<unsigned char, false>));
+    MM_CUDA_TRY(cudaFuncGetAttributes(&attr, prep_float_operands_kernel));
+    MM_CUDA_TRY(cudaFuncGetAttributes(&attr, complete_tf32_kernel));
+    MM_CUDA_TRY(cudaFuncGetAttributes(&attr, transpose_prep_kernel<__half>));
+    MM_CUDA_TRY(cudaFuncGetAttributes(&attr, transpose_prep_kernel<unsigned char>));
     if (!get_encode_fn()) return fail(MM_ERR_CUDA, "cuTensorMapEncodeTiled entry point not available");
     return gemm_dispatch(dtype, nullptr, nullptr, nullptr, g.n, g.k, g.m, g.flags, t, nullptr, nullptr, 0, true, g.stream,
                          g.batch, g.accumulate);
@@ -633,15 +883,25 @@ int launch_tcgen05(int dtype, const GemmArgs &g, void *scratch, size_t scratch_b
   PreparedB pb;
   const void *a_op = nullptr;
   const HalfScratch hs = tcgen05_half_scratch(scratch, scratch_bytes, dtype, g.n, g.k, g.m, g.flags, t, g.batch);
-  if (hs.fits_b) MM_CUDA_TRY(cudaMemsetAsync(hs.fits_b, 1, hs.flag_bytes, g.stream));  // every operand fits until seen
-  // one preparation pass per operand for the whole batch; a shared operand is prepared once
-  int rc = tcgen05_prepare_b_async(dtype, src, nullptr, scratch, scratch_bytes, g.k, g.m, g.flags, t, g.stream,
-                                   g.side_stream, g.ev_fork, g.ev_join, &pb, g.batch.b_copies(), hs.b, hs.fits_b);
-  if (rc == MM_OK) {
-    rc = tcgen05_prepare_a(dtype, g.a, aprep, g.n, g.k, g.flags, t, &a_op, g.stream, g.batch.a_copies(), hs.a,
-                           hs.fits_a);
+  // the whole batch is prepared at once; a shared operand is prepared once
+  int rc = MM_OK;
+  if (hs.fits_b) {
+    // every operand fits and every item's TF32 copy is owed until seen; then one pass over A and B
+    MM_CUDA_TRY(cudaMemsetAsync(hs.fits_b, 1, hs.flag_bytes, g.stream));
+    pb.b_op = scratch;
+    a_op = aprep;
+    rc = tcgen05_prepare_float(false, g.a, 0, g.n, g.b, g.n, g.k, g.m, g.flags, t, g.batch, scratch, scratch_bytes,
+                               g.stream);
+  } else {
+    rc = tcgen05_prepare_b_async(dtype, src, nullptr, scratch, scratch_bytes, g.k, g.m, g.flags, t, g.stream,
+                                 g.side_stream, g.ev_fork, g.ev_join, &pb, g.batch.b_copies());
+    if (rc == MM_OK) rc = tcgen05_prepare_a(dtype, g.a, aprep, g.n, g.k, g.flags, t, &a_op, g.stream, g.batch.a_copies());
   }
   if (rc == MM_OK && g.agree != nullptr) rc = (*g.agree)(hs.fits_a, g.stream);
+  if (rc == MM_OK && hs.fits_b) {  // the words are final: the TF32 copies still owed
+    rc = tcgen05_prepare_float(true, g.a, 0, g.n, g.b, g.n, g.k, g.m, g.flags, t, g.batch, scratch, scratch_bytes,
+                               g.stream);
+  }
   if (rc == MM_OK && g.ev_prep_done) cudaEventRecord(g.ev_prep_done, g.stream);
   if (rc == MM_OK) {
     rc = tcgen05_gemm(dtype, a_op, pb.b_op, g.c, g.n, g.k, g.m, g.flags, t, cnt.tile_sync, pb.ready, pb.ready_target,
