@@ -89,10 +89,9 @@ Tuning default_tuning() {
 struct mm_context {
   int device = 0;
   cudaStream_t stream = nullptr;
-  cudaStream_t side = nullptr;                         // B's operand preparation, overlapped with the GEMM
   cudaStream_t copy_in = nullptr, copy_out = nullptr;  // H2D / D2H streams of the pipelined host path
   std::vector<cudaEvent_t> sync_events;                // untimed events ordering the streams
-  cudaEvent_t ev_start = nullptr, ev_stop = nullptr, ev_fork = nullptr, ev_join = nullptr;
+  cudaEvent_t ev_start = nullptr, ev_stop = nullptr;
   cudaEvent_t ev_slice = nullptr;                      // multi-GPU: this device's slice of B has arrived
   mm::Scratch scratch;       // operand copies of the tensor-core path
   mm::Scratch staging[3];    // device A, B, C of the host-pointer entries
@@ -186,9 +185,6 @@ mm::GemmArgs make_args(mm_context *ctx, const void *a, const void *b, void *c, u
                        int flags, cudaStream_t stream) {
   mm::GemmArgs g{a, b, c, n, k, m, flags, stream};
   g.tuning = &ctx->tuning;
-  g.side_stream = ctx->side;
-  g.ev_fork = ctx->ev_fork;
-  g.ev_join = ctx->ev_join;
   return g;
 }
 
@@ -259,10 +255,7 @@ int enqueue_locked(mm_context *ctx, int dtype, int map_op, int reduce_op, int fl
   cudaEvent_t *pe;
   const int rc_begin = begin_call(ctx, stream, !dry_run, &capture, &pe);
   if (rc_begin != MM_OK) return rc_begin;
-  if (pe) {
-    g.ev_start = pe[0];
-    g.ev_prep_done = pe[1];
-  }
+  if (pe) g.ev_prep_done = pe[1];
   int rc_launch = MM_OK;
   switch (select_path(dtype, map_op, reduce_op, flags, n, k)) {
     case kPathTcgen05: {
@@ -294,7 +287,6 @@ int enqueue_locked(mm_context *ctx, int dtype, int map_op, int reduce_op, int fl
 void destroy_context(mm_context *ctx) {
   cudaSetDevice(ctx->device);
   if (ctx->stream) cudaStreamSynchronize(ctx->stream);
-  if (ctx->side) cudaStreamSynchronize(ctx->side);
   if (ctx->scratch.ptr) cudaFree(ctx->scratch.ptr);
   for (auto &s : ctx->staging) {
     if (s.ptr) cudaFree(s.ptr);
@@ -302,10 +294,10 @@ void destroy_context(mm_context *ctx) {
   for (void *p : ctx->retired) cudaFree(p);
   for (auto e : ctx->prof_events) cudaEventDestroy(e);
   for (auto e : ctx->sync_events) cudaEventDestroy(e);
-  for (cudaEvent_t e : {ctx->ev_start, ctx->ev_stop, ctx->ev_fork, ctx->ev_join, ctx->ev_slice}) {
+  for (cudaEvent_t e : {ctx->ev_start, ctx->ev_stop, ctx->ev_slice}) {
     if (e) cudaEventDestroy(e);
   }
-  for (cudaStream_t s : {ctx->copy_in, ctx->copy_out, ctx->side, ctx->stream}) {
+  for (cudaStream_t s : {ctx->copy_in, ctx->copy_out, ctx->stream}) {
     if (s) cudaStreamDestroy(s);
   }
   delete ctx;
@@ -313,13 +305,10 @@ void destroy_context(mm_context *ctx) {
 
 int init_context(mm_context *ctx) {
   MM_CUDA_TRY(cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking));
-  MM_CUDA_TRY(cudaStreamCreateWithFlags(&ctx->side, cudaStreamNonBlocking));
   MM_CUDA_TRY(cudaStreamCreateWithFlags(&ctx->copy_in, cudaStreamNonBlocking));
   MM_CUDA_TRY(cudaStreamCreateWithFlags(&ctx->copy_out, cudaStreamNonBlocking));
   MM_CUDA_TRY(cudaEventCreate(&ctx->ev_start));
   MM_CUDA_TRY(cudaEventCreate(&ctx->ev_stop));
-  MM_CUDA_TRY(cudaEventCreateWithFlags(&ctx->ev_fork, cudaEventDisableTiming));
-  MM_CUDA_TRY(cudaEventCreateWithFlags(&ctx->ev_join, cudaEventDisableTiming));
   MM_CUDA_TRY(cudaEventCreateWithFlags(&ctx->ev_slice, cudaEventDisableTiming));
   return MM_OK;
 }
@@ -327,11 +316,11 @@ int init_context(mm_context *ctx) {
 // ---- the pipelined host-pointer path --------------------------------------------------------------
 // How B reaches the device of one pipeline.  Single GPU: the whole of B over PCIe.  Multi-GPU: this
 // device uploads rows [k0, k1) only; the other slices are read from the peers' B buffers over NVLink
-// (`parts_dev`: device array of `parts` base pointers, slice j = rows [j * part_rows, ...)).
+// (`parts_dev`: device array of the devices' B base pointers, slice j = rows [j * part_rows, ...)).
 struct BPlan {
   unsigned k0 = 0, k1 = 0;
   const void *const *parts_dev = nullptr;
-  unsigned parts = 1, part_rows = 0;
+  unsigned part_rows = 0;
   std::vector<cudaEvent_t> peer_slices;  // the peers' "slice uploaded" events (recorded before this is used)
 };
 
@@ -370,15 +359,14 @@ struct Pipeline {
   // Phase 2: A row-chunks in, kernels, C row-chunks out; blocking.  C row-blocks are independent
   // (kernel/Compute.cpp:53-56), so the H2D copy of A chunk i+1, the kernels of chunk i and the D2H
   // copy of C chunk i-1 run concurrently on three streams; B is assembled (and, on the tcgen05 path,
-  // prepared — overlapped with the first chunk's GEMM) once.  A stored K x N cannot be cut into
-  // contiguous row chunks: single chunk.
+  // prepared) once.  A stored K x N cannot be cut into contiguous row chunks: single chunk.
   // `agree` (multi-GPU, mm::AgreeFn): called once every A chunk of this device is prepared and before any GEMM.
   int run(const BPlan &bp, double *seconds_device, const mm::AgreeFn *agree = nullptr) {
     const int rc = enqueue_all(bp, agree);
     // drain every stream before returning, on the error paths too: the caller's host buffers must
     // not be touched by copies in flight after this call has returned
     cudaError_t e = cudaSuccess;
-    for (cudaStream_t s : {ctx->copy_in, ctx->side, ctx->stream, ctx->copy_out}) {
+    for (cudaStream_t s : {ctx->copy_in, ctx->stream, ctx->copy_out}) {
       const cudaError_t es_ = cudaStreamSynchronize(s);
       if (e == cudaSuccess) e = es_;
     }
@@ -432,37 +420,27 @@ struct Pipeline {
     MM_CUDA_TRY(cudaStreamWaitEvent(ctx->stream, ctx->ev_slice, 0));
     for (cudaEvent_t e : bp.peer_slices) MM_CUDA_TRY(cudaStreamWaitEvent(ctx->stream, e, 0));
     MM_CUDA_TRY(cudaEventRecord(ctx->ev_start, ctx->stream));
-    mm::BSource src;
-    src.b = db;
-    if (bp.parts_dev != nullptr) {  // also with a single slice: the GPUs that did not upload it read it from its owner
-      src.src = bp.parts_dev;
-      src.parts = bp.parts;
-      src.part_rows = bp.part_rows;
-    }
     int rc = MM_OK;
-    mm::PreparedB pb;
+    if (bp.parts_dev != nullptr) {  // also with a single slice: the GPUs that did not upload it read it from its owner
+      rc = mm::gather_b_rows(bp.parts_dev, bp.part_rows, db, es, k, m, ctx->stream);  // the peers' slices, over NVLink
+      if (rc != MM_OK) return rc;
+    }
+    const void *b_op = nullptr;
     unsigned char *aprep = nullptr;
     mm::HalfScratch hs;
     if (path == kPathTcgen05) {
       hs = mm::tcgen05_half_scratch(ctx->scratch.ptr, ctx->scratch.bytes, dtype, rows, k, m, flags, t);
       if (hs.fits_b) {
-        // float: the one-pass preparation of B from this GPU's whole B (the peers' slices gathered in first)
+        // float: the one-pass preparation of B
         MM_CUDA_TRY(cudaMemsetAsync(hs.fits_b, 1, hs.flag_bytes, ctx->stream));
-        if (bp.parts_dev != nullptr) rc = mm::gather_b_rows(src, db, es, k, m, ctx->stream);
-        if (rc == MM_OK) {
-          rc = mm::tcgen05_prepare_float(false, nullptr, 0, 0, db, rows, k, m, flags, t, mm::GemmBatch{},
-                                         ctx->scratch.ptr, ctx->scratch.bytes, ctx->stream);
-        }
-        pb.b_op = ctx->scratch.ptr;
+        rc = mm::tcgen05_prepare_float(false, nullptr, 0, 0, db, rows, k, m, flags, t, mm::GemmBatch{},
+                                       ctx->scratch.ptr, ctx->scratch.bytes, ctx->stream);
+        b_op = ctx->scratch.ptr;
       } else {
-        rc = mm::tcgen05_prepare_b_async(dtype, src, db, ctx->scratch.ptr, ctx->scratch.bytes, k, m, flags, t,
-                                         ctx->stream, ctx->side, ctx->ev_fork, ctx->ev_join, &pb, 1);
+        rc = mm::tcgen05_prepare_b(dtype, db, ctx->scratch.ptr, k, m, flags, t, &b_op, ctx->stream);
       }
       if (rc != MM_OK) return rc;
       aprep = static_cast<unsigned char *>(ctx->scratch.ptr) + mm::tcgen05_bt_bytes(dtype, k, m, flags, t);
-    } else if (bp.parts_dev != nullptr) {
-      rc = mm::gather_b_rows(src, db, es, k, m, ctx->stream);  // the peers' slices into this GPU's B, over NVLink
-      if (rc != MM_OK) return rc;
     }
     // With fp16 copies every chunk's preparation clears the one fits flag of A, and the GEMMs start once all of A is
     // prepared and the TF32 copies still owed are written: each chunk then takes the datapath of the whole A, so the
@@ -491,9 +469,9 @@ struct Pipeline {
       if (path == kPathTcgen05) {
         mm::HalfOperands half = hs.operands();
         if (half.a) half.a = static_cast<const unsigned char *>(half.a) + r0 * k * 2;
-        const mm::Tcgen05Counters cnt = mm::tcgen05_counters(ctx->scratch.ptr, ctx->scratch.bytes);
-        rc1 = mm::tcgen05_gemm(dtype, a_ops[i], pb.b_op, c_chunk, unsigned(nr), k, m, flags, t, cnt.tile_sync, pb.ready,
-                               pb.ready_target, ctx->stream, mm::GemmBatch{}, false, half);
+        rc1 = mm::tcgen05_gemm(dtype, a_ops[i], b_op, c_chunk, unsigned(nr), k, m, flags, t,
+                               mm::tcgen05_tile_sync(ctx->scratch.ptr, ctx->scratch.bytes), ctx->stream,
+                               mm::GemmBatch{}, false, half);
       } else {
         mm::GemmArgs g = make_args(ctx, a_chunk, db, c_chunk, unsigned(nr), k, m, flags, ctx->stream);
         rc1 = (path == kPathDmma) ? mm::launch_dmma(g) : mm::launch_semiring(dtype, map_op, reduce_op, g);
@@ -513,7 +491,6 @@ struct Pipeline {
       if (!prepare_first) rc = prepare(i);
       if (rc == MM_OK) rc = compute(i);
     }
-    if (path == kPathTcgen05 && pb.forked) cudaStreamWaitEvent(ctx->stream, ctx->ev_join, 0);
     if (rc != MM_OK) return rc;
     MM_CUDA_TRY(cudaEventRecord(ctx->ev_stop, ctx->stream));
 
@@ -689,7 +666,6 @@ int multi_gemm_host_locked(mm_multi *mu, int dtype, int map_op, int reduce_op, i
     bp.k0 = part.k0;
     bp.k1 = part.k1;
     if (mu->peer) {
-      bp.parts = part.parts;
       bp.part_rows = part.part_rows;
       bp.parts_dev = mu->parts_dev[g];
     }
@@ -1071,12 +1047,10 @@ int mm_context_profile_read(mm_context *ctx, double *prep_sum, double *main_sum,
 
 int mm_kernel_launch_count(int dtype, int map_op, int reduce_op, int flags) {
   if (!valid_dtype(dtype) || !valid_op(map_op) || !valid_op(reduce_op)) return -1;
-  const mm::Tuning t = mm::default_tuning();
   switch (select_path(dtype, map_op, reduce_op, flags, 2, 64)) {
     case kPathTcgen05:
-      // [B preparation unless B is read in place] + [A preparation for float or transposed A] + GEMM
-      return 1 + (mm::tcgen05_b_in_place(dtype, flags, t) ? 0 : 1) +
-             ((dtype == MM_DTYPE_FLOAT || (flags & MM_FLAG_TRANSPOSED_A)) ? 1 : 0);
+      // B's preparation + [float's second preparation pass, or A's transpose] + GEMM
+      return 2 + ((dtype == MM_DTYPE_FLOAT || (flags & MM_FLAG_TRANSPOSED_A)) ? 1 : 0);
     case kPathDmma: return 1;
     case kPathSemiring: return 1;
   }
@@ -1222,7 +1196,7 @@ int mm_multi_upload(mm_multi *mu, int dtype, int flags, const void *a, const voi
     std::lock_guard<std::mutex> ctx_lock(ctx->mutex);
     gen[g] = ++ctx->staging_gen;
     const Partition part = partition_for(G, g, n, k, mu->peer);
-    const unsigned r0 = part.r0, r1 = part.r1, part_rows = part.part_rows, parts = part.parts;
+    const unsigned r0 = part.r0, r1 = part.r1, part_rows = part.part_rows;
     const unsigned rows = std::max(1u, r1 - r0);
     auto body = [&]() -> int {
       MM_CUDA_TRY(cudaSetDevice(ctx->device));
@@ -1257,11 +1231,7 @@ int mm_multi_upload(mm_multi *mu, int dtype, int flags, const void *a, const voi
         for (int j = 0; j < G; ++j) {
           if (j != g) MM_CUDA_TRY(cudaStreamWaitEvent(ctx->stream, mu->ctx[j]->ev_slice, 0));
         }
-        mm::BSource src;
-        src.src = mu->parts_dev[g];
-        src.parts = parts;
-        src.part_rows = part_rows;
-        return mm::gather_b_rows(src, ctx->staging[1].ptr, es, k, m, ctx->stream);
+        return mm::gather_b_rows(mu->parts_dev[g], part_rows, ctx->staging[1].ptr, es, k, m, ctx->stream);
       };
       rc2 = gather();
     }

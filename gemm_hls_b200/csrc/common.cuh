@@ -49,9 +49,7 @@ struct Tuning {
   int stages() const { return v[MM_TUNE_TCGEN05_STAGES]; }
   int raster_rows() const { return v[MM_TUNE_TCGEN05_RASTER_ROWS]; }
   bool tile_sync() const { return v[MM_TUNE_TCGEN05_TILE_SYNC] != 0; }
-  bool b_mn() const { return v[MM_TUNE_TCGEN05_B_MN] != 0; }
   int l2_policy() const { return v[MM_TUNE_TCGEN05_L2_POLICY]; }
-  int b_overlap() const { return v[MM_TUNE_TCGEN05_B_OVERLAP]; }
   bool tma_store() const { return v[MM_TUNE_TCGEN05_TMA_STORE] != 0; }
   int dmma_tile_rows() const { return v[MM_TUNE_DMMA_TILE_ROWS]; }
   bool tf32_no_round() const { return v[MM_TUNE_EXPERIMENT_TF32_NO_ROUND] != 0; }
@@ -79,13 +77,8 @@ struct GemmArgs {
   cudaStream_t stream;
   const Tuning *tuning = nullptr;  // never null on a real launch (capi.cu fills it from the context)
   GemmBatch batch;
-  // Second stream + fork/join events of the context: B's operand preparation runs there, overlapped
-  // with the GEMM that consumes it panel by panel (gemm_tcgen05.cu).  Null = no overlap.
-  cudaStream_t side_stream = nullptr;
-  cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
-  // optional profiling events (capi.cu): recorded by the launcher between operand preparation
+  // optional profiling event (capi.cu): recorded by the launcher between operand preparation
   // and the main kernel when non-null
-  cudaEvent_t ev_start = nullptr;
   cudaEvent_t ev_prep_done = nullptr;
   // Resource-preparation pass: do everything a launch does EXCEPT enqueue kernels (set function
   // attributes, which also forces the lazily loaded cubin in).  mm_kernel_execute runs it before
@@ -106,7 +99,7 @@ int launch_semiring_witness(int dtype, int map_op, int reduce_op, const GemmArgs
 int launch_semiring_accumulate(int dtype, int map_op, int reduce_op, const GemmArgs &args);
 
 // wgmma tensor-core GEMM for (Multiply, Add) float (tf32), half (f16) and uint8_t (u8).
-// The context's scratch holds, in this order: [B operand copy][B fp16][A operand copy][A fp16] ... [fits][counters].
+// The context's scratch holds, in this order: [B operand copy][B fp16][A operand copy][A fp16] ... [fits][wave-barrier counter].
 //   B operand copy: the transposed M x K copy wgmma reads K-major, rounded to TF32 for float.
 //   A operand copy: float = A rounded to TF32; any type with MM_FLAG_TRANSPOSED_A = A transposed.
 //   fp16 copies and fits flags (float on the default TF32 datapath only, see HalfScratch): the rounded copies again as
@@ -123,7 +116,7 @@ struct HalfOperands {
   const void *a = nullptr, *b = nullptr;
   const unsigned int *fits_a = nullptr, *fits_b = nullptr;
 };
-// Where the preparation writes them.  Just before the counters at the scratch's end: [one fits word per B copy][one per
+// Where the preparation writes them.  Just before the wave-barrier counter at the scratch's end: [one fits word per B copy][one per
 // A copy][pending map of B][pending map of A], all set nonzero by one cudaMemsetAsync of flag_bytes before the
 // preparation.  A fits word is cleared by any preparation item that meets a value which is not exactly a normal half or
 // zero (fits_half.h).  The pending maps hold one byte per 64 x 64 item of each copy: 1 while the item's TF32 copy is
@@ -138,52 +131,16 @@ struct HalfScratch {
 };
 HalfScratch tcgen05_half_scratch(void *scratch, size_t scratch_bytes, int dtype, unsigned n, unsigned k, unsigned m,
                                  int flags, const Tuning &t, const GemmBatch &batch = GemmBatch{});
-// How the kernel consumes B for this configuration.
-bool tcgen05_b_mn(int dtype, int flags, const Tuning &t);      // MN-major (row-major K x M array) vs K-major copy
-bool tcgen05_b_in_place(int dtype, int flags, const Tuning &t);  // no B copy at all (half, MN-major)
-
 // The phases of launch_tcgen05, for callers that reuse a prepared B across row-blocks (the pipelined
 // host path, the multi-GPU row-block driver).
-// Where the kernel's B operand comes from.  `src` non-null: `parts` row-slices of B of `part_rows`
-// rows each (the last may be short), slice j read through src[j] — a pointer to a FULL-size K x M
-// array of which only slice j's rows need to be valid (peer-GPU buffers of the multi-GPU path: the
-// NVLink all-gather of B is fused into this pass).  `src` null: one array, `b`.
-struct BSource {
-  const void *b = nullptr;
-  const void *const *src = nullptr;  // DEVICE array of `parts` pointers
-  unsigned parts = 1;
-  unsigned part_rows = 0;
-};
-// Counters at the tail of the scratch (zeroed by the launchers before use).
-struct Tcgen05Counters {
-  unsigned int *tile_sync;  // soft wave barrier of the GEMM
-  unsigned int *b_ready;    // one per BLOCK_N-column panel of B: finished preparation work items
-};
-Tcgen05Counters tcgen05_counters(void *scratch, size_t scratch_bytes);
-// Prepares B into `bt` on `stream`.  *b_op receives the kernel's B operand (bt, or the caller's B when
-// it is read in place).  With `ready` non-null the pass runs panel by panel (BLOCK_N columns of B at
-// a time, in the order the GEMM's rasterisation consumes them) as a co-resident persistent kernel and
-// publishes each panel through ready[panel]; *ready_target receives the count that means "complete".
-// `copies` packed K x M problems of B are prepared into `copies` packed M x K copies (K-major path only).
-// Not for float on the default datapath: see tcgen05_prepare_float.
-int tcgen05_prepare_b(int dtype, const BSource &src, void *bt, unsigned k, unsigned m, int flags, const Tuning &t,
-                      const void **b_op, unsigned int *ready, unsigned *ready_target, cudaStream_t stream,
-                      unsigned copies = 1);
-// Fork / join wrapper around tcgen05_prepare_b for the launchers: decides whether the preparation
-// overlaps the GEMM (float rounding, or any gather of peer slices, with the MN-major B path and a side
-// stream), zeroes the panel counters in stream order, runs the pass on `side` — ENQUEUED BEFORE the
-// GEMM that waits on its counters, so that serialising tools (ncu, compute-sanitizer) still run it
-// first — and records `ev_join` there.  `local_b`: where a plain gather of slices goes when B needs no
-// scratch copy (half); may be null for a single source.
-struct PreparedB {
-  const void *b_op = nullptr;
-  const unsigned int *ready = nullptr;  // pass to tcgen05_gemm
-  unsigned ready_target = 0;
-  bool forked = false;  // the caller makes `stream` wait on `ev_join` after its last GEMM
-};
-int tcgen05_prepare_b_async(int dtype, const BSource &src, void *local_b, void *scratch, size_t scratch_bytes,
-                            unsigned k, unsigned m, int flags, const Tuning &t, cudaStream_t stream, cudaStream_t side,
-                            cudaEvent_t ev_fork, cudaEvent_t ev_join, PreparedB *out, unsigned copies = 1);
+// The soft wave-barrier counter of the GEMM, at the tail of the scratch (zeroed by the launcher before use).
+unsigned int *tcgen05_tile_sync(void *scratch, size_t scratch_bytes);
+// The K-major copy of B (M x K, one K x M array `b` per copy) into `bt` on `stream`: the hi / lo split for
+// MM_FLAG_TF32X3, the unrounded transpose for float under the tf32_no_round experiment, the transpose for half,
+// bfloat16 and uint8_t.  *b_op receives the kernel's B operand (bt).  `copies` packed K x M problems of B are prepared
+// into `copies` packed M x K copies.  Not for float on the default datapath: see tcgen05_prepare_float.
+int tcgen05_prepare_b(int dtype, const void *b, void *bt, unsigned k, unsigned m, int flags, const Tuning &t,
+                      const void **b_op, cudaStream_t stream, unsigned copies = 1);
 // `copies` packed problems of `rows` rows each.  Not for float on the default datapath: see tcgen05_prepare_float.
 int tcgen05_prepare_a(int dtype, const void *a, void *aprep, unsigned rows, unsigned k, int flags, const Tuning &t,
                       const void **a_op, cudaStream_t stream, unsigned copies = 1);
@@ -196,16 +153,17 @@ int tcgen05_prepare_a(int dtype, const void *a, void *aprep, unsigned rows, unsi
 int tcgen05_prepare_float(bool complete, const void *a, unsigned row0, unsigned rows, const void *b, unsigned n,
                           unsigned k, unsigned m, int flags, const Tuning &t, const GemmBatch &batch, void *scratch,
                           size_t scratch_bytes, cudaStream_t stream);
-// `tile_sync`: device counter for the kernel's soft wave barrier, or null.  `b_ready` non-null: the
-// producer waits for b_ready[column tile] >= b_ready_target before it fetches a tile's B panel.
+// `tile_sync`: device counter for the kernel's soft wave barrier, or null.
 int tcgen05_gemm(int dtype, const void *a_op, const void *b_op, void *c, unsigned rows, unsigned k, unsigned m,
-                 int flags, const Tuning &t, unsigned int *tile_sync, const unsigned int *b_ready,
-                 unsigned b_ready_target, cudaStream_t stream, const GemmBatch &batch = GemmBatch{},
-                 bool accumulate = false, const HalfOperands &half = HalfOperands{});
-constexpr size_t kTcgen05TailBytes = 256 + 64 * 1024;  // [panel counters, 64 KiB][wave-barrier counter, 256 B]
-// Generic gather of row-sliced B into one local array (identity transform): what the multi-GPU path
-// uses for the kernel families that read B as is (double, semirings, half).
-int gather_b_rows(const BSource &src, void *dst, size_t elem_bytes, unsigned k, unsigned m, cudaStream_t stream);
+                 int flags, const Tuning &t, unsigned int *tile_sync, cudaStream_t stream,
+                 const GemmBatch &batch = GemmBatch{}, bool accumulate = false,
+                 const HalfOperands &half = HalfOperands{});
+constexpr size_t kTcgen05TailBytes = 256;  // [wave-barrier counter, 256 B]
+// The NVLink all-gather of the multi-GPU path, for every kernel family: row-sliced B into one local K x M array
+// `dst`.  K-row r is read through parts[r / part_rows], a DEVICE array of pointers to FULL-size K x M arrays (the
+// devices' B buffers) of which only that slice's rows need to be valid; rows already in `dst` are not copied.
+int gather_b_rows(const void *const *parts, unsigned part_rows, void *dst, size_t elem_bytes, unsigned k, unsigned m,
+                  cudaStream_t stream);
 
 // DMMA (mma.sync m8n8k4 f64) GEMM for (Multiply, Add) double.  gemm_dmma.cu
 int launch_dmma(const GemmArgs &args);

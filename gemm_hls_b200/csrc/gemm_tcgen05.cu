@@ -25,13 +25,16 @@
 //   * tf32 wgmma reads only the upper 19 bits of each fp32 operand, i.e. it TRUNCATES.  The
 //     reference's inputs are all positive (U[1,10], test/TestSimulation.cpp:46-55), so truncation
 //     would bias every product by about -2^-11 * 2 and land the sum right at the 1e-3 tolerance.
-//     A and B are therefore rounded to nearest TF32 (cvt.rna.tf32.f32) into scratch copies first.
-//   * half, bfloat16 and uint8_t A are K-major as stored; B is transposed.  bfloat16 moves the same bits as
-//     half, so it shares half's transpose kernel.
-//   * A value rounded to TF32 keeps 10 mantissa bits, as many as a half has.  So the same passes also write the
-//     rounded operands as halves and note, per distinct operand, whether every value is 0 or a normal half
+//     Float A and B are therefore rounded to nearest TF32 (cvt.rna.tf32.f32) into scratch copies first, by
+//     prep_float_operands_kernel and complete_tf32_kernel.
+//   * A value rounded to TF32 keeps 10 mantissa bits, as many as a half has.  So those passes may write the
+//     rounded operands as halves instead, and note, per distinct operand, whether every value is 0 or a normal half
 //     (fits_half.h).  A problem whose A and B both fit runs on the f16 wgmma, which multiplies the very same values
 //     at twice the TF32 issue rate (gemm_wgmma.cuh); any other problem stays on TF32.
+//   * MM_FLAG_TF32X3 splits float A and B into hi / lo parts (split3_*); the tf32_no_round experiment transposes
+//     float B unrounded.
+//   * half, bfloat16 and uint8_t A are K-major as stored; B is transposed.  bfloat16 moves the same bits as
+//     half, so it shares half's transpose kernel.
 //
 // The GEMM kernel and its launcher are in gemm_wgmma.cuh.  This unit instantiates them for tf32, f16 and
 // u8; the bf16 instantiations are in gemm_wgmma_bf16.cu, the accumulate kernels in gemm_wgmma_acc.cu.
@@ -68,22 +71,6 @@ __device__ __forceinline__ float round_tf32(float x) {
 __device__ __forceinline__ uint32_t half2_bits(float lo, float hi) {
   const __half2 h = __floats2half2_rn(lo, hi);
   return *reinterpret_cast<const uint32_t *>(&h);
-}
-
-// dst[i] = rna_tf32(src[i]); count4 float4 per problem, blockIdx.y = problem of a batch (packed).
-__global__ void __launch_bounds__(256)
-round_tf32_kernel(const float4 *__restrict__ src, float4 *__restrict__ dst, size_t count4) {
-  src += size_t(blockIdx.y) * count4;
-  dst += size_t(blockIdx.y) * count4;
-  const size_t stride = size_t(gridDim.x) * blockDim.x;
-  for (size_t i = size_t(blockIdx.x) * blockDim.x + threadIdx.x; i < count4; i += stride) {
-    float4 v = src[i];
-    v.x = round_tf32(v.x);
-    v.y = round_tf32(v.y);
-    v.z = round_tf32(v.z);
-    v.w = round_tf32(v.w);
-    dst[i] = v;
-  }
 }
 
 // ---- float on the default datapath: one preparation pass that writes the copy the GEMM will read ---------------
@@ -310,73 +297,50 @@ complete_tf32_kernel(const FloatPrepArgs args) {
   }
 }
 
-// B (row-major K x M, 16-byte vectors) -> dst (same layout), panel by panel: a work item is
-// PANEL_ROWS k-rows of one panel of `panel_v` vectors per row; items are numbered panel-major and
-// dealt round-robin to the CTAs of a persistent grid, so panels complete in ascending order.  Each
-// finished item bumps ready[panel] (release pattern: every thread fences its stores, the CTA syncs,
-// one thread adds).  ROUND: elements are floats rounded to nearest TF32; otherwise a plain copy.
-// `parts` non-null: k-row r is read from parts[r / part_rows] — full-size K x M arrays on (peer) GPUs
-// of which only that slice of rows is valid; rows whose source IS the destination are skipped.
-constexpr int PREP_THREADS = 512;
-constexpr int PREP_WARPS = PREP_THREADS / 32;
-constexpr int PANEL_ROWS = 64;
-constexpr int PANEL_ROW_SLOTS = PANEL_ROWS / PREP_WARPS;  // rows per warp per item (4)
+// Row-sliced B (row-major K x M, 16-byte vectors) -> dst (same layout): k-row r is read from parts[r / part_rows], a
+// full-size K x M array on a (peer) GPU of which only that slice of rows is valid; rows whose source IS the
+// destination are skipped.  A work item is GATHER_ROWS k-rows of GATHER_VECS vectors (1 KiB) per row, 8 loads in
+// flight per thread; items are numbered column-block-major and dealt round-robin to the CTAs of a persistent grid.
+constexpr int GATHER_THREADS = 512;
+constexpr int GATHER_WARPS = GATHER_THREADS / 32;
+constexpr int GATHER_ROWS = 64;
+constexpr int GATHER_VECS = 64;
+constexpr int GATHER_ROW_SLOTS = GATHER_ROWS / GATHER_WARPS;  // rows per warp per item (4)
 
-template <bool ROUND>
-__device__ __forceinline__ uint4 prep_vec(uint4 v) {
-  if (ROUND) {
-    v.x = __float_as_uint(round_tf32(__uint_as_float(v.x)));
-    v.y = __float_as_uint(round_tf32(__uint_as_float(v.y)));
-    v.z = __float_as_uint(round_tf32(__uint_as_float(v.z)));
-    v.w = __float_as_uint(round_tf32(__uint_as_float(v.w)));
-  }
-  return v;
-}
-
-template <bool ROUND>
-__global__ void __launch_bounds__(PREP_THREADS)
-prep_b_panels_kernel(const uint4 *__restrict__ single, const uint4 *const *__restrict__ parts, uint32_t part_rows,
-                     uint4 *__restrict__ dst, uint32_t k, uint32_t row_v, uint32_t panel_v,
-                     unsigned int *__restrict__ ready) {
+__global__ void __launch_bounds__(GATHER_THREADS)
+gather_rows_kernel(const uint4 *const *__restrict__ parts, uint32_t part_rows, uint4 *__restrict__ dst, uint32_t k,
+                   uint32_t row_v) {
   const uint32_t warp = threadIdx.x / 32, lane = threadIdx.x % 32;
-  const uint32_t panels = (row_v + panel_v - 1) / panel_v;
-  const uint32_t items_per_panel = (k + PANEL_ROWS - 1) / PANEL_ROWS;
-  const uint32_t items = panels * items_per_panel;
+  const uint32_t col_blocks = (row_v + GATHER_VECS - 1) / GATHER_VECS;
+  const uint32_t items_per_col_block = (k + GATHER_ROWS - 1) / GATHER_ROWS;
+  const uint32_t items = col_blocks * items_per_col_block;
   for (uint32_t item = blockIdx.x; item < items; item += gridDim.x) {
-    const uint32_t panel = item / items_per_panel;
-    const uint32_t r0 = (item - panel * items_per_panel) * PANEL_ROWS;
-    const uint32_t v0 = panel * panel_v;
-    const uint32_t w = min(panel_v, row_v - v0);
-    for (uint32_t c0 = 0; c0 < w; c0 += 64) {   // 64 vectors (1 KiB) of a row per pass: 8 loads in flight per thread
-      uint4 buf[PANEL_ROW_SLOTS][2];
-      bool live[PANEL_ROW_SLOTS][2];
+    const uint32_t col_block = item / items_per_col_block;
+    const uint32_t r0 = (item - col_block * items_per_col_block) * GATHER_ROWS;
+    const uint32_t v0 = col_block * GATHER_VECS;
+    const uint32_t w = min(uint32_t(GATHER_VECS), row_v - v0);
+    uint4 buf[GATHER_ROW_SLOTS][2];
+    bool live[GATHER_ROW_SLOTS][2];
 #pragma unroll
-      for (int u = 0; u < PANEL_ROW_SLOTS; ++u) {
-        const uint32_t r = r0 + warp + u * PREP_WARPS;
-        const uint4 *src = single;
-        if (parts != nullptr && r < k) src = parts[r / part_rows];
+    for (int u = 0; u < GATHER_ROW_SLOTS; ++u) {
+      const uint32_t r = r0 + warp + u * GATHER_WARPS;
+      const uint4 *src = r < k ? parts[r / part_rows] : nullptr;
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const uint32_t c = c0 + lane + 32 * h;
-          const size_t off = size_t(r) * row_v + v0 + c;
-          live[u][h] = (r < k) && (c < w) && (src + off != static_cast<const uint4 *>(dst) + off);
-          if (live[u][h]) buf[u][h] = src[off];
-        }
-      }
-#pragma unroll
-      for (int u = 0; u < PANEL_ROW_SLOTS; ++u) {
-        const uint32_t r = r0 + warp + u * PREP_WARPS;
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const uint32_t c = c0 + lane + 32 * h;
-          if (live[u][h]) dst[size_t(r) * row_v + v0 + c] = prep_vec<ROUND>(buf[u][h]);
-        }
+      for (int h = 0; h < 2; ++h) {
+        const uint32_t c = lane + 32 * h;
+        const size_t off = size_t(r) * row_v + v0 + c;
+        live[u][h] = (r < k) && (c < w) && (src != dst);
+        if (live[u][h]) buf[u][h] = src[off];
       }
     }
-    if (ready != nullptr) {
-      __threadfence();
-      __syncthreads();
-      if (threadIdx.x == 0) atomicAdd(ready + panel, 1u);
+#pragma unroll
+    for (int u = 0; u < GATHER_ROW_SLOTS; ++u) {
+      const uint32_t r = r0 + warp + u * GATHER_WARPS;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const uint32_t c = lane + 32 * h;
+        if (live[u][h]) dst[size_t(r) * row_v + v0 + c] = buf[u][h];
+      }
     }
   }
 }
@@ -500,55 +464,16 @@ void launch_transpose(const void *src, void *dst, uint32_t src_rows, uint32_t sr
                                                      src_cols);
 }
 
-// Rounds `copies` packed problems of count4 float4 each.
-int launch_round(const void *src, void *dst, size_t count4, unsigned copies, cudaStream_t stream) {
-  const int blocks = int(std::min<size_t>((count4 + 255) / 256, size_t(num_sms()) * 16));
-  const dim3 grid(std::max(blocks, 1), copies);
-  // see tcgen05_prepare_b
-  MM_CUDA_TRY(cudaFuncSetAttribute(round_tf32_kernel, cudaFuncAttributePreferredSharedMemoryCarveout,
-                                   cudaSharedmemCarveoutMaxShared));
-  round_tf32_kernel<<<grid, 256, 0, stream>>>(static_cast<const float4 *>(src), static_cast<float4 *>(dst), count4);
-  return MM_OK;
-}
-
 bool split3(int dtype, int flags) { return dtype == MM_DTYPE_FLOAT && (flags & MM_FLAG_TF32X3); }
-
-int launch_panels(bool round, const BSource &src, void *dst, size_t elem_bytes, unsigned k, unsigned m,
-                  unsigned panel_cols, unsigned int *ready, int grid, cudaStream_t stream) {
-  const uint32_t row_v = uint32_t(size_t(m) * elem_bytes / 16);
-  const uint32_t panel_v = uint32_t(size_t(panel_cols) * elem_bytes / 16);
-  const uint4 *single = static_cast<const uint4 *>(src.b);
-  const uint4 *const *parts = reinterpret_cast<const uint4 *const *>(src.src);
-  if (round) {
-    prep_b_panels_kernel<true><<<grid, PREP_THREADS, 0, stream>>>(single, parts, src.part_rows, static_cast<uint4 *>(dst),
-                                                                 k, row_v, panel_v, ready);
-  } else {
-    prep_b_panels_kernel<false><<<grid, PREP_THREADS, 0, stream>>>(single, parts, src.part_rows, static_cast<uint4 *>(dst),
-                                                                  k, row_v, panel_v, ready);
-  }
-  MM_CUDA_TRY(cudaGetLastError());
-  return MM_OK;
-}
 
 }  // namespace
 
-// Tail of the scratch: [panel counters of B's preparation, 64 KiB][soft wave-barrier counter, 256 B]
-constexpr size_t TILE_SYNC_BYTES = 256;
-constexpr size_t B_READY_BYTES = 64 * 1024;  // 16384 panels of >= 128 columns
-constexpr size_t TAIL_BYTES = TILE_SYNC_BYTES + B_READY_BYTES;
+// Tail of the scratch: the soft wave-barrier counter of the GEMM, 256 B
+constexpr size_t TAIL_BYTES = 256;
 static_assert(TAIL_BYTES == kTcgen05TailBytes, "common.cuh and gemm_tcgen05.cu disagree on the scratch tail");
 
-Tcgen05Counters tcgen05_counters(void *scratch, size_t scratch_bytes) {
-  unsigned char *tail = static_cast<unsigned char *>(scratch) + scratch_bytes;
-  return Tcgen05Counters{reinterpret_cast<unsigned int *>(tail - TILE_SYNC_BYTES),
-                         reinterpret_cast<unsigned int *>(tail - TAIL_BYTES)};
-}
-
-// wgmma reads tf32 and 8-bit operands only K-major; every type takes the K-major copy of B.
-bool tcgen05_b_mn(int, int, const Tuning &) { return false; }
-
-bool tcgen05_b_in_place(int dtype, int flags, const Tuning &t) {
-  return tcgen05_b_mn(dtype, flags, t) && (dtype == MM_DTYPE_HALF || dtype == MM_DTYPE_UINT8 || t.tf32_no_round());
+unsigned int *tcgen05_tile_sync(void *scratch, size_t scratch_bytes) {
+  return reinterpret_cast<unsigned int *>(static_cast<unsigned char *>(scratch) + scratch_bytes - TAIL_BYTES);
 }
 
 // float on the default TF32 datapath: the preparation also writes fp16 copies and fits flags (HalfScratch)
@@ -573,14 +498,13 @@ size_t fits_bytes(unsigned n, unsigned k, unsigned m, const GemmBatch &batch) {
 }
 
 size_t tcgen05_bt_bytes(int dtype, unsigned k, unsigned m, int flags, const Tuning &t, unsigned b_copies) {
-  if (tcgen05_b_in_place(dtype, flags, t)) return 0;
   const size_t fp16 = half_copies(dtype, flags, t) ? align_up(size_t(b_copies) * m * k * 2, 1024) : 0;
   return b_copy_bytes(dtype, k, m, flags, b_copies) + fp16;  // [B copy][B fp16]
 }
 
 size_t tcgen05_scratch_bytes(int dtype, unsigned n, unsigned k, unsigned m, int flags, const Tuning &t,
                              const GemmBatch &batch) {
-  size_t bytes = TAIL_BYTES + tcgen05_bt_bytes(dtype, k, m, flags, t, batch.b_copies());  // counters (tail) + B copies
+  size_t bytes = TAIL_BYTES + tcgen05_bt_bytes(dtype, k, m, flags, t, batch.b_copies());  // counter (tail) + B copies
   bytes += a_copy_bytes(dtype, n, k, flags, batch.a_copies());
   if (half_copies(dtype, flags, t)) bytes += align_up(size_t(batch.a_copies()) * n * k * 2, 1024) + fits_bytes(n, k, m, batch);
   return bytes;
@@ -602,58 +526,18 @@ HalfScratch tcgen05_half_scratch(void *scratch, size_t scratch_bytes, int dtype,
   return h;
 }
 
-// Copy row-sliced B (slices on peer GPUs) into one local array: the NVLink all-gather of the
-// multi-GPU path for the kernel families that consume B as stored.
-int gather_b_rows(const BSource &src, void *dst, size_t elem_bytes, unsigned k, unsigned m, cudaStream_t stream) {
-  return launch_panels(false, src, dst, elem_bytes, k, m, /*panel_cols=*/unsigned(1024 / elem_bytes), nullptr,
-                       num_sms() * 2, stream);
+int gather_b_rows(const void *const *parts, unsigned part_rows, void *dst, size_t elem_bytes, unsigned k, unsigned m,
+                  cudaStream_t stream) {
+  const uint32_t row_v = uint32_t(size_t(m) * elem_bytes / 16);
+  gather_rows_kernel<<<num_sms() * 2, GATHER_THREADS, 0, stream>>>(reinterpret_cast<const uint4 *const *>(parts),
+                                                                   part_rows, static_cast<uint4 *>(dst), k, row_v);
+  MM_CUDA_TRY(cudaGetLastError());
+  return MM_OK;
 }
 
-int tcgen05_prepare_b(int dtype, const BSource &src, void *bt, unsigned k, unsigned m, int flags, const Tuning &t,
-                      const void **b_op, unsigned int *ready, unsigned *ready_target, cudaStream_t stream,
-                      unsigned copies) {
+int tcgen05_prepare_b(int dtype, const void *b, void *bt, unsigned k, unsigned m, int flags, const Tuning &t,
+                      const void **b_op, cudaStream_t stream, unsigned copies) {
   *b_op = bt;
-  if (ready_target) *ready_target = 0;
-  const bool parts = src.src != nullptr;
-  const size_t eb = elem_bytes(dtype);
-  if (tcgen05_b_mn(dtype, flags, t)) {
-    if (copies != 1) return fail(MM_ERR_UNSUPPORTED, "batched calls need the K-major B copy");
-    const bool in_place = tcgen05_b_in_place(dtype, flags, t);
-    if (in_place && !parts) {
-      *b_op = src.b;  // nothing to prepare
-      return MM_OK;
-    }
-    // float: rounded copy (same layout).  half / unrounded float with slices: plain gather into `bt`.
-    if (!in_place && !parts && ready == nullptr) {
-      // one local array, nobody waiting on panels: the flat elementwise pass (6.3 TB/s against the panel
-      // kernel's 5.1 on a 512 MiB block — the panel order costs row-segment locality)
-      const int rc = launch_round(src.b, bt, size_t(k) * m / 4, 1, stream);
-      if (rc != MM_OK) return rc;
-      MM_CUDA_TRY(cudaGetLastError());
-      return MM_OK;
-    }
-    const unsigned panel_cols = unsigned(t.block_n());
-    const unsigned panels = ceil_div(m, panel_cols);
-    const bool publish = ready != nullptr && panels <= B_READY_BYTES / sizeof(unsigned int);
-    if (publish && ready_target) *ready_target = ceil_div(k, PANEL_ROWS);
-    // co-resident persistent grid (one 512-thread CTA per SM next to the GEMM's CTA) when the GEMM
-    // consumes panels while this runs; a wider grid when it runs alone in stream order
-    const int grid = publish ? num_sms() : num_sms() * 2;
-    // An SM changes its L1 / shared-memory split only when it is idle.  This kernel uses no shared memory; were it
-    // to run under the default (L1-heavy) split, the GEMM's CTAs (214 KiB of shared memory) could not become
-    // resident next to it and would wait for it to END — measured: the "overlapped" GEMM took exactly its own time
-    // plus this kernel's.  Ask for the shared-memory-heavy split so that both fit on an SM together.
-    // (Function attributes are per device: set on every call, it is cheap.  A's rounding kernel may share SMs with
-    // this one, so it asks for the same split — tcgen05_prepare_a.)
-    MM_CUDA_TRY(cudaFuncSetAttribute(prep_b_panels_kernel<true>, cudaFuncAttributePreferredSharedMemoryCarveout,
-                                     cudaSharedmemCarveoutMaxShared));
-    MM_CUDA_TRY(cudaFuncSetAttribute(prep_b_panels_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout,
-                                     cudaSharedmemCarveoutMaxShared));
-    return launch_panels(!in_place, src, bt, eb, k, m, panel_cols, publish ? ready : nullptr, grid, stream);
-  }
-  // K-major copy B^T (M x K): tuning knob b_mn = 0, and always for the 3xTF32 split
-  const void *b = src.b;
-  if (parts) return fail(MM_ERR_UNSUPPORTED, "row-sliced B needs the MN-major B path (gather it first)");
   if (split3(dtype, flags)) {
     dim3 grid((m + 63) / 64, (k + 63) / 64, copies);
     split3_transpose_kernel<true><<<grid, 256, 0, stream>>>(static_cast<const float *>(b), static_cast<float *>(bt), k, m);
@@ -781,23 +665,20 @@ int tcgen05_prepare_float(bool complete, const void *a, unsigned row0, unsigned 
 
 namespace {
 int gemm_dispatch(int dtype, const void *a_op, const void *b_op, void *c, unsigned rows, unsigned k, unsigned m,
-                  int flags, const Tuning &t, unsigned int *tile_sync, const unsigned int *b_ready,
-                  unsigned b_ready_target, bool attributes_only, cudaStream_t stream, const GemmBatch &batch,
-                  bool accumulate = false, const HalfOperands &half = HalfOperands{}) {
+                  int flags, const Tuning &t, unsigned int *tile_sync, bool attributes_only, cudaStream_t stream,
+                  const GemmBatch &batch, bool accumulate = false, const HalfOperands &half = HalfOperands{}) {
   if (accumulate) {
     if (split3(dtype, flags)) k *= 3;
-    return wgmma_accumulate_gemm(dtype, a_op, b_op, c, rows, k, m, t, tile_sync, b_ready, b_ready_target,
-                                 attributes_only, stream, batch, half);
+    return wgmma_accumulate_gemm(dtype, a_op, b_op, c, rows, k, m, t, tile_sync, attributes_only, stream, batch, half);
   }
   if (dtype == MM_DTYPE_BFLOAT16) {
-    return wgmma_bf16_gemm(a_op, b_op, c, rows, k, m, t, tile_sync, b_ready, b_ready_target, attributes_only, stream,
-                           batch);
+    return wgmma_bf16_gemm(a_op, b_op, c, rows, k, m, t, tile_sync, attributes_only, stream, batch);
   }
   if (split3(dtype, flags)) k *= 3;  // the operands carry [hi|hi|lo] x [hi|lo|hi] per 16-block of K
   CUtensorMap maps[5];
   LaunchPlan plan;
-  const int rc = plan_gemm(dtype, a_op, b_op, c, rows, k, m, t, tile_sync, b_ready, b_ready_target, attributes_only,
-                           stream, batch, half, maps, &plan);
+  const int rc = plan_gemm(dtype, a_op, b_op, c, rows, k, m, t, tile_sync, attributes_only, stream, batch, half, maps,
+                           &plan);
   if (rc != MM_OK) return rc;
   const int cg = t.cta_group(), bn = t.block_n();
   if (dtype == MM_DTYPE_UINT8) return dispatch_variant<ptx::KIND_I8, unsigned char>(cg, bn, plan);
@@ -810,46 +691,9 @@ int gemm_dispatch(int dtype, const void *a_op, const void *b_op, void *c, unsign
 // C[rows x m] = Aop[rows x k] * B on the tensor cores; `b_op` as returned by tcgen05_prepare_b.  `accumulate`:
 // C <- C + that product, by the accumulate kernels.  `half`: float's fp16 copies and fits flags, or empty.
 int tcgen05_gemm(int dtype, const void *a_op, const void *b_op, void *c, unsigned rows, unsigned k, unsigned m,
-                 int flags, const Tuning &t, unsigned int *tile_sync, const unsigned int *b_ready,
-                 unsigned b_ready_target, cudaStream_t stream, const GemmBatch &batch, bool accumulate,
-                 const HalfOperands &half) {
-  return gemm_dispatch(dtype, a_op, b_op, c, rows, k, m, flags, t, tile_sync, b_ready, b_ready_target, false, stream,
-                       batch, accumulate, half);
-}
-
-int tcgen05_prepare_b_async(int dtype, const BSource &src, void *local_b, void *scratch, size_t scratch_bytes,
-                            unsigned k, unsigned m, int flags, const Tuning &t, cudaStream_t stream, cudaStream_t side,
-                            cudaEvent_t ev_fork, cudaEvent_t ev_join, PreparedB *out, unsigned copies) {
-  *out = PreparedB{};
-  const bool in_place = tcgen05_b_in_place(dtype, flags, t);
-  const bool parts = src.src != nullptr;
-  if (copies != 1) {
-    if (parts) return fail(MM_ERR_UNSUPPORTED, "batched calls take B from one array");
-    return tcgen05_prepare_b(dtype, src, scratch, k, m, flags, t, &out->b_op, nullptr, nullptr, stream, copies);
-  }
-  if (parts && !tcgen05_b_mn(dtype, flags, t)) {
-    // K-major copy requested (tuning / 3xTF32): assemble the slices first, then transpose locally
-    int rc = gather_b_rows(src, local_b, elem_bytes(dtype), k, m, stream);
-    if (rc != MM_OK) return rc;
-    BSource whole;
-    whole.b = local_b;
-    return tcgen05_prepare_b(dtype, whole, scratch, k, m, flags, t, &out->b_op, nullptr, nullptr, stream, 1);
-  }
-  void *bt = in_place ? local_b : scratch;
-  const Tcgen05Counters cnt = tcgen05_counters(scratch, scratch_bytes);
-  const unsigned panels = ceil_div(m, unsigned(t.block_n()));
-  // the panel kernel runs (float rounding, or a gather of slices), a second stream exists, the tuning allows it
-  const bool overlap = side != nullptr && t.b_overlap() != 0 && tcgen05_b_mn(dtype, flags, t) && (!in_place || parts) &&
-                       panels <= B_READY_BYTES / sizeof(unsigned int);
-  if (!overlap) return tcgen05_prepare_b(dtype, src, bt, k, m, flags, t, &out->b_op, nullptr, nullptr, stream, 1);
-  MM_CUDA_TRY(cudaMemsetAsync(cnt.b_ready, 0, panels * sizeof(unsigned int), stream));
-  MM_CUDA_TRY(cudaEventRecord(ev_fork, stream));
-  MM_CUDA_TRY(cudaStreamWaitEvent(side, ev_fork, 0));
-  const int rc = tcgen05_prepare_b(dtype, src, bt, k, m, flags, t, &out->b_op, cnt.b_ready, &out->ready_target, side);
-  cudaEventRecord(ev_join, side);  // the side stream rejoins whatever happened above
-  out->forked = true;
-  out->ready = cnt.b_ready;
-  return rc;
+                 int flags, const Tuning &t, unsigned int *tile_sync, cudaStream_t stream, const GemmBatch &batch,
+                 bool accumulate, const HalfOperands &half) {
+  return gemm_dispatch(dtype, a_op, b_op, c, rows, k, m, flags, t, tile_sync, false, stream, batch, accumulate, half);
 }
 
 int launch_tcgen05(int dtype, const GemmArgs &g, void *scratch, size_t scratch_bytes) {
@@ -861,40 +705,33 @@ int launch_tcgen05(int dtype, const GemmArgs &g, void *scratch, size_t scratch_b
   if (g.dry_run) {
     // force the lazily loaded kernels in (prep + the GEMM variant this tuning selects) and the driver entry point
     cudaFuncAttributes attr;
-    MM_CUDA_TRY(cudaFuncGetAttributes(&attr, round_tf32_kernel));
-    MM_CUDA_TRY(cudaFuncGetAttributes(&attr, prep_b_panels_kernel<true>));
-    MM_CUDA_TRY(cudaFuncGetAttributes(&attr, prep_b_panels_kernel<false>));
+    MM_CUDA_TRY(cudaFuncGetAttributes(&attr, gather_rows_kernel));
     MM_CUDA_TRY(cudaFuncGetAttributes(&attr, prep_float_operands_kernel));
     MM_CUDA_TRY(cudaFuncGetAttributes(&attr, complete_tf32_kernel));
     MM_CUDA_TRY(cudaFuncGetAttributes(&attr, transpose_prep_kernel<__half>));
     MM_CUDA_TRY(cudaFuncGetAttributes(&attr, transpose_prep_kernel<unsigned char>));
     if (!get_encode_fn()) return fail(MM_ERR_CUDA, "cuTensorMapEncodeTiled entry point not available");
-    return gemm_dispatch(dtype, nullptr, nullptr, nullptr, g.n, g.k, g.m, g.flags, t, nullptr, nullptr, 0, true, g.stream,
-                         g.batch, g.accumulate);
+    return gemm_dispatch(dtype, nullptr, nullptr, nullptr, g.n, g.k, g.m, g.flags, t, nullptr, true, g.stream, g.batch,
+                         g.accumulate);
   }
   if (scratch_bytes < tcgen05_scratch_bytes(dtype, g.n, g.k, g.m, g.flags, t, g.batch)) {
     return fail(MM_ERR_INVALID, "tcgen05 scratch too small");
   }
   unsigned char *sp = static_cast<unsigned char *>(scratch);
   void *aprep = sp + tcgen05_bt_bytes(dtype, g.k, g.m, g.flags, t, g.batch.b_copies());
-  const Tcgen05Counters cnt = tcgen05_counters(scratch, scratch_bytes);
-  BSource src;
-  src.b = g.b;
-  PreparedB pb;
-  const void *a_op = nullptr;
+  const void *a_op = nullptr, *b_op = nullptr;
   const HalfScratch hs = tcgen05_half_scratch(scratch, scratch_bytes, dtype, g.n, g.k, g.m, g.flags, t, g.batch);
   // the whole batch is prepared at once; a shared operand is prepared once
   int rc = MM_OK;
   if (hs.fits_b) {
     // every operand fits and every item's TF32 copy is owed until seen; then one pass over A and B
     MM_CUDA_TRY(cudaMemsetAsync(hs.fits_b, 1, hs.flag_bytes, g.stream));
-    pb.b_op = scratch;
+    b_op = scratch;
     a_op = aprep;
     rc = tcgen05_prepare_float(false, g.a, 0, g.n, g.b, g.n, g.k, g.m, g.flags, t, g.batch, scratch, scratch_bytes,
                                g.stream);
   } else {
-    rc = tcgen05_prepare_b_async(dtype, src, nullptr, scratch, scratch_bytes, g.k, g.m, g.flags, t, g.stream,
-                                 g.side_stream, g.ev_fork, g.ev_join, &pb, g.batch.b_copies());
+    rc = tcgen05_prepare_b(dtype, g.b, scratch, g.k, g.m, g.flags, t, &b_op, g.stream, g.batch.b_copies());
     if (rc == MM_OK) rc = tcgen05_prepare_a(dtype, g.a, aprep, g.n, g.k, g.flags, t, &a_op, g.stream, g.batch.a_copies());
   }
   if (rc == MM_OK && g.agree != nullptr) rc = (*g.agree)(hs.fits_a, g.stream);
@@ -904,10 +741,9 @@ int launch_tcgen05(int dtype, const GemmArgs &g, void *scratch, size_t scratch_b
   }
   if (rc == MM_OK && g.ev_prep_done) cudaEventRecord(g.ev_prep_done, g.stream);
   if (rc == MM_OK) {
-    rc = tcgen05_gemm(dtype, a_op, pb.b_op, g.c, g.n, g.k, g.m, g.flags, t, cnt.tile_sync, pb.ready, pb.ready_target,
+    rc = tcgen05_gemm(dtype, a_op, b_op, g.c, g.n, g.k, g.m, g.flags, t, tcgen05_tile_sync(scratch, scratch_bytes),
                       g.stream, g.batch, g.accumulate, hs.operands());
   }
-  if (pb.forked) cudaStreamWaitEvent(g.stream, g.ev_join, 0);  // join, on the error paths too
   return rc;
 }
 

@@ -160,11 +160,6 @@ __device__ __forceinline__ uint32_t cluster_ctarank() {
 __device__ __forceinline__ void cluster_sync_all() {
   asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
-__device__ __forceinline__ unsigned int ld_acquire_gpu(const unsigned int *p) {
-  unsigned int v;
-  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-  return v;
-}
 
 // Run-time launch parameters of the GEMM kernel (one struct so that the instantiations share a
 // signature).
@@ -173,14 +168,12 @@ struct GemmParams {
   uint32_t num_stages;       // ring depth actually used (<= Geo::MAX_STAGES, what the smem allocation holds)
   uint32_t raster_group;     // row tiles per rasterisation group
   uint32_t tma_store;        // 1: staged TMA-store epilogue, 0: direct stores
-  uint32_t b_ready_target;   // see b_ready
   // Batch: `batch` problems of rows x cols.  A and B are read through 2-D maps with the problems
   // stacked along the row dimension: problem i starts at row i * a_prob_rows of A and
   // i * b_prob_rows of B (0 = every problem reads the same operand).  C is a 3-D map {cols, rows, batch}.
   uint32_t batch, a_prob_rows, b_prob_rows;
   uint64_t l2_policy;
   unsigned int *tile_sync;        // soft wave-barrier counter or null
-  const unsigned int *b_ready;    // per column tile: preparation items finished, or null (B complete)
   // float only: per distinct A (B) operand of the batch, nonzero when every TF32-rounded value of it is exactly a half
   // (gemm_tcgen05.cu); a tile whose A and B both fit reads the fp16 copies and runs on the f16 wgmma.  Null: TF32 only.
   const unsigned int *fits_a, *fits_b;
@@ -254,7 +247,6 @@ __device__ __forceinline__ void gemm_wgmma_body(const CUtensorMap &tmap_a, const
     if (threadIdx.x == 0) {
       uint32_t stage = 0, phase = 0;
       uint32_t tile_iter = 0;
-      int32_t ready_panel = -1;
       for (uint32_t t = group_id; t < num_tiles; t += num_groups, ++tile_iter) {
         // Soft wave barrier: do not start fetching tile #j before every CTA group has finished
         // fetching its tile #(j-1), so that co-running tiles keep sharing their A / B panels in L2.
@@ -271,17 +263,6 @@ __device__ __forceinline__ void gemm_wgmma_body(const CUtensorMap &tmap_a, const
         // that are never stored.  K is the inner dimension, so the K tail is zero-filled per row.
         const int32_t a_row = tc.prob * p.a_prob_rows + tc.r * G::TILE_ROWS + cta_rank * BLOCK_M;
         const int32_t b_row = tc.prob * p.b_prob_rows + tc.c * BN + cta_rank * G::LOAD_N;
-        if (p.b_ready != nullptr && int32_t(tc.c) != ready_panel) {
-          // B's preparation kernel was ENQUEUED before this kernel and needs no resource this kernel
-          // holds, so it always makes progress; the bound only turns an impossible wait into a trap.
-          const unsigned int *flag = p.b_ready + tc.c;
-          const long long t0 = clock64();
-          while (ld_acquire_gpu(flag) < p.b_ready_target) {
-            if (clock64() - t0 > (1ll << 34)) __trap();
-          }
-          asm volatile("fence.proxy.async.global;" ::: "memory");  // generic-proxy writes -> TMA reads
-          ready_panel = int32_t(tc.c);
-        }
         const bool h = half_tile(tc);
         const CUtensorMap *map_a = h ? &tmap_a16 : &tmap_a;
         const CUtensorMap *map_b = h ? &tmap_b16 : &tmap_b;
@@ -590,13 +571,11 @@ int dispatch_variant(int cg, int bn, const LaunchPlan &plan) {
 // (A, B, C, fp16 A, fp16 B) must outlive the launch; `k` is the K extent the operands carry.  `half`: float's fp16
 // operand copies and fits flags (gemm_tcgen05.cu), or empty.
 int plan_gemm(int dtype, const void *a_op, const void *b_op, void *c, unsigned rows, unsigned k, unsigned m,
-              const Tuning &t, unsigned int *tile_sync, const unsigned int *b_ready, unsigned b_ready_target,
-              bool attributes_only, cudaStream_t stream, const GemmBatch &batch, const HalfOperands &half,
-              CUtensorMap (&maps)[5], LaunchPlan *plan) {
+              const Tuning &t, unsigned int *tile_sync, bool attributes_only, cudaStream_t stream,
+              const GemmBatch &batch, const HalfOperands &half, CUtensorMap (&maps)[5], LaunchPlan *plan) {
   const size_t eb = elem_bytes(dtype);
   const int cg = t.cta_group(), bn = t.block_n();
   const bool use_half = dtype == MM_DTYPE_FLOAT && half.fits_a != nullptr;
-  if (batch.count > 1 && b_ready != nullptr) return fail(MM_ERR_UNSUPPORTED, "batched calls need a complete B operand");
   std::memset(&maps[2], 0, sizeof(maps[2]));
   *plan = LaunchPlan{&maps[0], &maps[1], &maps[2], use_half ? &maps[3] : &maps[0], use_half ? &maps[4] : &maps[1],
                      c, {}, t.stages(), attributes_only, stream};
@@ -626,10 +605,8 @@ int plan_gemm(int dtype, const void *a_op, const void *b_op, void *c, unsigned r
   p.k_bytes = uint32_t(size_t(k) * eb);
   p.raster_group = uint32_t(std::max(1, t.raster_rows()));  // in rows here; per-variant tiles in the launcher
   p.tma_store = t.tma_store() ? 1u : 0u;
-  p.b_ready_target = b_ready_target;
   p.l2_policy = t.l2_policy() == 1 ? ptx::L2_EVICT_FIRST : (t.l2_policy() == 2 ? ptx::L2_EVICT_LAST : ptx::L2_EVICT_NORMAL);
   p.tile_sync = t.tile_sync() ? tile_sync : nullptr;
-  p.b_ready = b_ready;
   p.fits_a = use_half ? half.fits_a : nullptr;
   p.fits_b = use_half ? half.fits_b : nullptr;
   return MM_OK;
@@ -640,14 +617,12 @@ int plan_gemm(int dtype, const void *a_op, const void *b_op, void *c, unsigned r
 // bf16 (Multiply, Add): the four bf16 instantiations of the kernel live in their own translation unit,
 // gemm_wgmma_bf16.cu.  Arguments as gemm_dispatch in gemm_tcgen05.cu.
 int wgmma_bf16_gemm(const void *a_op, const void *b_op, void *c, unsigned rows, unsigned k, unsigned m, const Tuning &t,
-                    unsigned int *tile_sync, const unsigned int *b_ready, unsigned b_ready_target, bool attributes_only,
-                    cudaStream_t stream, const GemmBatch &batch);
+                    unsigned int *tile_sync, bool attributes_only, cudaStream_t stream, const GemmBatch &batch);
 
 // C <- C + product for every type of the wgmma path (mm_kernel_enqueue_accumulate): the sixteen accumulate kernels
 // live in gemm_wgmma_acc.cu.  `k` is the K extent the operands carry (3K for 3xTF32).
 int wgmma_accumulate_gemm(int dtype, const void *a_op, const void *b_op, void *c, unsigned rows, unsigned k, unsigned m,
-                          const Tuning &t, unsigned int *tile_sync, const unsigned int *b_ready,
-                          unsigned b_ready_target, bool attributes_only, cudaStream_t stream, const GemmBatch &batch,
-                          const HalfOperands &half);
+                          const Tuning &t, unsigned int *tile_sync, bool attributes_only, cudaStream_t stream,
+                          const GemmBatch &batch, const HalfOperands &half);
 
 }  // namespace mm

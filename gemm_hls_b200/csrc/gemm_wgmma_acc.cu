@@ -10,13 +10,12 @@
 namespace mm {
 
 int wgmma_accumulate_gemm(int dtype, const void *a_op, const void *b_op, void *c, unsigned rows, unsigned k, unsigned m,
-                          const Tuning &t, unsigned int *tile_sync, const unsigned int *b_ready,
-                          unsigned b_ready_target, bool attributes_only, cudaStream_t stream, const GemmBatch &batch,
-                          const HalfOperands &half) {
+                          const Tuning &t, unsigned int *tile_sync, bool attributes_only, cudaStream_t stream,
+                          const GemmBatch &batch, const HalfOperands &half) {
   CUtensorMap maps[5];
   LaunchPlan plan;
-  const int rc = plan_gemm(dtype, a_op, b_op, c, rows, k, m, t, tile_sync, b_ready, b_ready_target, attributes_only,
-                           stream, batch, half, maps, &plan);
+  const int rc = plan_gemm(dtype, a_op, b_op, c, rows, k, m, t, tile_sync, attributes_only, stream, batch, half, maps,
+                           &plan);
   if (rc != MM_OK) return rc;
   const int cg = t.cta_group(), bn = t.block_n();
   switch (dtype) {

@@ -9,12 +9,11 @@
 namespace mm {
 
 int wgmma_bf16_gemm(const void *a_op, const void *b_op, void *c, unsigned rows, unsigned k, unsigned m, const Tuning &t,
-                    unsigned int *tile_sync, const unsigned int *b_ready, unsigned b_ready_target, bool attributes_only,
-                    cudaStream_t stream, const GemmBatch &batch) {
+                    unsigned int *tile_sync, bool attributes_only, cudaStream_t stream, const GemmBatch &batch) {
   CUtensorMap maps[5];
   LaunchPlan plan;
-  const int rc = plan_gemm(MM_DTYPE_BFLOAT16, a_op, b_op, c, rows, k, m, t, tile_sync, b_ready, b_ready_target,
-                           attributes_only, stream, batch, HalfOperands{}, maps, &plan);
+  const int rc = plan_gemm(MM_DTYPE_BFLOAT16, a_op, b_op, c, rows, k, m, t, tile_sync, attributes_only, stream, batch,
+                           HalfOperands{}, maps, &plan);
   if (rc != MM_OK) return rc;
   return dispatch_variant<ptx::KIND_BF16, __nv_bfloat16>(t.cta_group(), t.block_n(), plan);
 }

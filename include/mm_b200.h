@@ -290,8 +290,8 @@ enum {
   MM_TUNE_TCGEN05_B_MN = 5,        /* 0 | 1: accepted, no effect on sm_90a: wgmma reads tf32 and 8-bit
                                       operands only K-major, so B is always a transposed copy         MM_TCGEN05_B_MN */
   MM_TUNE_TCGEN05_L2_POLICY = 6,   /* TMA loads' L2 eviction priority: 0 normal, 1 first, 2 last       MM_TCGEN05_L2 */
-  MM_TUNE_TCGEN05_B_OVERLAP = 7,   /* 0 | 1: accepted, no effect on sm_90a (B's preparation overlaps the
-                                      GEMM only when B is read in its row-major layout)                MM_TCGEN05_B_OVERLAP */
+  MM_TUNE_TCGEN05_B_OVERLAP = 7,   /* 0 | 1: accepted, no effect on sm_90a: B's preparation always
+                                      completes before the GEMM starts                               MM_TCGEN05_B_OVERLAP */
   MM_TUNE_TCGEN05_TMA_STORE = 8,   /* 0 | 1: epilogue through shared memory + TMA stores (default 1)   MM_TCGEN05_TMA_STORE */
   MM_TUNE_DMMA_TILE_ROWS = 9,      /* 0 = automatic | 64 | 128: CTA tile rows of the double kernel     MM_DMMA_TILE_ROWS */
   MM_TUNE_EXPERIMENT_TF32_NO_ROUND = 10, /* 1: feed raw fp32 bits to tf32 wgmma (measures the truncation
@@ -319,10 +319,10 @@ MM_API int mm_context_reserve_batched(mm_context *ctx, int dtype, int flags, uns
  * and one device-resident lifecycle (host/RunHardware.cpp:116-190); outer tiles of C are independent
  * (kernel/Compute.cpp:53-56).  mm_multi keeps both shapes over G devices of this process: GPU g owns
  * rows [g*ceil(N/G), ...) of A and C; every GPU uploads only ITS 1/G row-slice of B over PCIe and the
- * slices are all-gathered GPU-to-GPU over NVLink by the library's own kernels reading peer memory —
- * fused with B's TF32 rounding on the float path, where the GEMM consumes finished panels while the
- * gather is still running.  No collective per step, no reduction (K is not split).  All fan-out is
- * internal (one host thread per GPU) and joined before the call returns.
+ * slices are all-gathered GPU-to-GPU over NVLink into each device's B by the library's own kernel
+ * reading peer memory, on every path; each device then prepares its B locally.  No collective per
+ * step, no reduction (K is not split).  All fan-out is internal (one host thread per GPU) and joined
+ * before the call returns.
  * A stored K x N (MM_FLAG_TRANSPOSED_A) cannot be cut into contiguous row blocks: MM_ERR_UNSUPPORTED. */
 typedef struct mm_multi mm_multi;
 /* `devices` = n_gpus CUDA ordinals, or NULL for 0 .. n_gpus-1. */

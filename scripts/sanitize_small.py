@@ -18,7 +18,7 @@ CASES = [
     ("wgmma_tf32", G.FLOAT, G.MULTIPLY, G.ADD, 0, (257, 48, 272)),
     ("wgmma_tf32 multi-tile", G.FLOAT, G.MULTIPLY, G.ADD, 0, (600, 80, 528)),
     ("wgmma_tf32 direct stores", G.FLOAT, G.MULTIPLY, G.ADD, 0, (257, 48, 272), dict(tma_store=0)),
-    ("wgmma_tf32 overlapped B", G.FLOAT, G.MULTIPLY, G.ADD, 0, (257, 48, 528), dict(b_overlap=1)),
+    ("wgmma_tf32 b_overlap=1 (no effect)", G.FLOAT, G.MULTIPLY, G.ADD, 0, (257, 48, 528), dict(b_overlap=1)),
     ("wgmma_tf32 K-major B, 1 CTA, 128 cols", G.FLOAT, G.MULTIPLY, G.ADD, 0, (257, 48, 272), dict(b_mn=0, cta_group=1, block_n=128)),
     ("wgmma_i8", G.UINT8, G.MULTIPLY, G.ADD, 0, (257, 192, 320)),
     ("wgmma_i8 TA, 1 CTA", G.UINT8, G.MULTIPLY, G.ADD, G.FLAG_TRANSPOSED_A, (130, 64, 192), dict(cta_group=1)),

@@ -298,7 +298,7 @@ def test_multi_lifecycle(mm, oracle, multis, name, gpus):
 @pytest.mark.parametrize("chunk", ["default", "128"])
 @pytest.mark.parametrize("name", ["tf32", "f16", "bf16", "u8", "dmma", "f32_add_min", "i32_mul_add", "u8_add_max"])
 def test_multi_on_distinct_devices(mm, oracle, multis, monkeypatch, name, chunk):
-    """B's slices cross NVLink: peer loads in the gather and in the fused preparation."""
+    """B's slices cross NVLink: peer loads in the gather."""
     fam = FAM[name]
     n, _, m = fam.shape
     _chunks(monkeypatch, chunk, n)

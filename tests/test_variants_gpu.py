@@ -8,7 +8,7 @@
   3. the multi-chunk pipeline of the host-pointer entry (test/TestSimulation.cpp:66 at sizes where
      A does not fit one chunk);
   4. the row-block split over several GPUs (mm_multi_*, SURVEY.md 8e) — on ONE device here by
-     listing it several times: slices of B, the gather kernel, panel counters and host barriers are
+     listing it several times: slices of B, the gather kernel, slice tables and host barriers are
      the same code that runs over NVLink;
   5. argument checks that need a device (alignment, tuning ranges, scratch growth under capture).
 """
@@ -314,7 +314,7 @@ def test_float_default_minmax_documented_exception(mm, oracle):
 # 3. the multi-chunk host pipeline
 # ---------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("dt,mp,rd,n,k,m", [
-    ("FLOAT", "MULTIPLY", "ADD", 1000, 512, 272),     # tcgen05: B prepared once (overlapped), 8 chunks of A
+    ("FLOAT", "MULTIPLY", "ADD", 1000, 512, 272),     # tcgen05: B prepared once, 8 chunks of A
     ("HALF", "MULTIPLY", "ADD", 700, 256, 160),
     ("DOUBLE", "MULTIPLY", "ADD", 520, 264, 136),     # DMMA
     ("FLOAT", "ADD", "MIN", 777, 64, 144),            # semiring
