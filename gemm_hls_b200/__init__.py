@@ -53,7 +53,7 @@ EXPORTS = ["mm_last_error", "mm_version", "mm_dtype_size", "mm_memory_width", "m
            "mm_kernel_enqueue_batched", "mm_context_reserve_batched", "mm_kernel_enqueue_witness",
            "mm_kernel_enqueue_accumulate", "mm_multi_create", "mm_multi_destroy", "mm_multi_device_count",
            "mm_multi_context", "mm_multi_peer_access", "mm_multi_partition", "mm_multi_gemm_host", "mm_multi_upload",
-           "mm_multi_execute", "mm_multi_download"]
+           "mm_multi_execute", "mm_multi_download", "mm_kernel_enqueue_closure", "mm_closure_block"]
 
 
 class MMError(RuntimeError):
@@ -100,6 +100,8 @@ def lib():
         L.mm_context_reserve_batched.argtypes = [vp, i, i, u, u, u, u]
         L.mm_kernel_enqueue_witness.argtypes = [vp, i, i, i, i, vp, vp, vp, vp, u, u, u, u, vp]
         L.mm_kernel_enqueue_accumulate.argtypes = [vp, i, i, i, i, vp, vp, vp, u, u, u, u, vp]
+        L.mm_kernel_enqueue_closure.argtypes = [vp, i, i, i, i, vp, u, u, vp]
+        L.mm_closure_block.argtypes, L.mm_closure_block.restype = [i], u
         L.mm_multi_create.argtypes = [i, ctypes.POINTER(i), ctypes.POINTER(vp)]
         L.mm_multi_destroy.argtypes = [vp]
         L.mm_multi_device_count.argtypes = [vp]
@@ -122,6 +124,11 @@ def _check(rc):
 
 def memory_width(dtype):
     return int(lib().mm_memory_width(dtype))
+
+
+def closure_block(dtype):
+    """b of Context.enqueue_closure: the width of its blocks of indices (0 for an unknown dtype)."""
+    return int(lib().mm_closure_block(dtype))
 
 
 def kernel_path(dtype, map_op=MULTIPLY, reduce_op=ADD, flags=0):
@@ -206,6 +213,13 @@ class Context:
         the call's reduce with the old C first (include/mm_b200.h).  C must not overlap A or B."""
         _check(lib().mm_kernel_enqueue_accumulate(self._h, dtype, map_op, reduce_op, flags, a_dev, b_dev, c_dev,
                                                   n, k, m, batch, ctypes.c_void_p(stream) if stream else None))
+
+    def enqueue_closure(self, dtype, map_op, reduce_op, d_dev, n, batch=1, flags=0, stream=None):
+        """D <- its closure over (map_op, reduce_op) in place, for `batch` packed n x n problems (reduce Min or Max):
+        blocked Floyd-Warshall with blocks of closure_block(dtype) indices, in the order include/mm_b200.h states.
+        The diagonal is not initialised."""
+        _check(lib().mm_kernel_enqueue_closure(self._h, dtype, map_op, reduce_op, flags, d_dev, n, batch,
+                                               ctypes.c_void_p(stream) if stream else None))
 
     def set_tuning(self, **knobs):
         """mm_context_set_tuning by name, e.g. ctx.set_tuning(cta_group=1, stages=4)."""

@@ -22,9 +22,9 @@ FLAGS = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-Xcompiler", 
          "--expt-relaxed-constexpr"]
 
 SOURCES = ["capi.cu", "gemm_tcgen05.cu", "gemm_wgmma_bf16.cu", "gemm_wgmma_acc.cu", "gemm_dmma.cu", "gemm_dmma_acc.cu",
-           "semiring_dispatch.cu", "semiring_witness_dispatch.cu"]
-# semiring_inst.cu, semiring_witness_inst.cu and semiring_accumulate_inst.cu are compiled once per (type, map
-# operator): (object suffix, C type)
+           "semiring_dispatch.cu", "semiring_witness_dispatch.cu", "semiring_closure_dispatch.cu"]
+# semiring_inst.cu, semiring_witness_inst.cu, semiring_accumulate_inst.cu and semiring_closure_inst.cu are compiled
+# once per (type, map operator): (object suffix, C type)
 INST_TYPES = [("f16", "__half"), ("f32", "float"), ("f64", "double"), ("i32", "int"),
               ("u32", "unsigned"), ("u8", "unsigned char"),
               ("bf16", "__nv_bfloat16")]
@@ -71,7 +71,8 @@ def build(force=False, verbose=False):
         jobs = [(src, obj % (suffix, mp), ["-DMM_INST_T=" + ctype, "-DMM_INST_MAP=%d" % mp])
                 for src, obj in (("semiring_inst.cu", "semiring_%s_%d.o"),
                                  ("semiring_witness_inst.cu", "semiring_witness_%s_%d.o"),
-                                 ("semiring_accumulate_inst.cu", "semiring_accumulate_%s_%d.o"))
+                                 ("semiring_accumulate_inst.cu", "semiring_accumulate_%s_%d.o"),
+                                 ("semiring_closure_inst.cu", "semiring_closure_%s_%d.o"))
                 for suffix, ctype in INST_TYPES for mp in INST_MAPS + ([5, 6] if suffix == "f32" else [])]
         jobs += [(src, src.replace(".cu", ".o"), []) for src in SOURCES]
         results = list(ex.map(lambda j: compile_one(j, force, verbose, hdr_time), jobs))

@@ -1010,6 +1010,34 @@ int mm_kernel_enqueue_witness(mm_context *ctx, int dtype, int map_op, int reduce
   return MM_OK;
 }
 
+unsigned mm_closure_block(int dtype) { return valid_dtype(dtype) ? 128u : 0u; }
+
+int mm_kernel_enqueue_closure(mm_context *ctx, int dtype, int map_op, int reduce_op, int flags, void *d, unsigned n,
+                              unsigned batch, void *cuda_stream) {
+  if (!ctx) return fail(MM_ERR_INVALID, "null context");
+  // D is A, B and C of an N x N x N problem: the witness call's checks with K = M = N
+  int rc = check_args(dtype, map_op, reduce_op, d, d, d, n, n, n);
+  if (rc != MM_OK) return rc;
+  if ((rc = check_batch(batch, n, n, n)) != MM_OK) return rc;
+  if ((rc = check_device_alignment(d, d, d)) != MM_OK) return rc;
+  if (reduce_op != MM_OP_MIN && reduce_op != MM_OP_MAX) {
+    return fail(MM_ERR_INVALID, "closures exist for the Min and Max reduces only");
+  }
+  if (flags & (MM_FLAG_TRANSPOSED_A | MM_FLAG_BATCH_SHARED_A | MM_FLAG_BATCH_SHARED_B)) {
+    return fail(MM_ERR_INVALID, "a closure takes neither MM_FLAG_TRANSPOSED_A nor MM_FLAG_BATCH_SHARED_A / _B");
+  }
+  std::lock_guard<std::mutex> lock(ctx->mutex);
+  MM_CUDA_TRY(cudaSetDevice(ctx->device));
+  cudaStream_t s = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ctx->stream;
+  cudaStreamCaptureStatus capture;
+  cudaEvent_t *pe;
+  if ((rc = begin_call(ctx, s, /*profile=*/true, &capture, &pe)) != MM_OK) return rc;
+  if (pe) MM_CUDA_TRY(cudaEventRecord(pe[1], s));  // like a semiring call: no preparation
+  if ((rc = mm::launch_semiring_closure(dtype, map_op, reduce_op, flags, d, n, batch, s)) != MM_OK) return rc;
+  if (pe) MM_CUDA_TRY(cudaEventRecord(pe[2], s));
+  return MM_OK;
+}
+
 int mm_kernel_execute(mm_context *ctx, int dtype, int map_op, int reduce_op, int flags,
                       const void *a, const void *b, void *c, unsigned n, unsigned k, unsigned m,
                       double *seconds_device, double *seconds_wall) {

@@ -97,6 +97,10 @@ int launch_semiring(int dtype, int map_op, int reduce_op, const GemmArgs &args);
 int launch_semiring_witness(int dtype, int map_op, int reduce_op, const GemmArgs &args, unsigned *w);
 // C <- Reduce(C_old, product) with the same kernel choice as launch_semiring.  semiring_accumulate_*.cu
 int launch_semiring_accumulate(int dtype, int map_op, int reduce_op, const GemmArgs &args);
+// Closure of `batch` packed N x N problems at d in place over a Min / Max reduce (mm_kernel_enqueue_closure), by
+// blocked Floyd–Warshall; float Min / Max take FMNMX unless MM_FLAG_EXACT.  semiring_closure_*.cu
+int launch_semiring_closure(int dtype, int map_op, int reduce_op, int flags, void *d, unsigned n, unsigned batch,
+                            cudaStream_t stream);
 
 // wgmma tensor-core GEMM for (Multiply, Add) float (tf32), half (f16) and uint8_t (u8).
 // The context's scratch holds, in this order: [B operand copy][B fp16][A operand copy][A fp16] ... [fits][wave-barrier counter].

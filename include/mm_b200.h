@@ -246,6 +246,43 @@ MM_API int mm_kernel_enqueue_accumulate(mm_context *ctx, int dtype, int map_op, 
                                         unsigned size_n, unsigned size_k, unsigned size_m,
                                         unsigned batch, void *cuda_stream);
 
+/* ---- closure: all-pairs shortest / longest / widest / most-reliable paths, reachability ------------------------
+ * mm_kernel_enqueue_closure() rewrites D in place: `batch` square N x N row-major matrices, packed (problem p starts
+ * at d_device + p*N*N elements), by blocked Floyd–Warshall over (Map, R), R = reduce_op = MM_OP_MIN or MM_OP_MAX.
+ * Asynchronous like the other enqueue entries.  It does NOT initialise the diagonal: callers who want reflexive paths
+ * set D[i][i] to the Map's identity themselves (0 for min-plus).
+ *
+ * b = mm_closure_block(dtype) = 128 for every type (the semiring kernels' CTA tile).  Blocks K_r = [r*b, min((r+1)*b,
+ * N)); the last may be partial, with a width that is a multiple of the memory width.  A "step k" updates its set of
+ * (i, j) simultaneously, every read of the step seeing the values from before it:
+ *     D'[i][j] = R(D[i][j], Map(D[i][k], D[k][j]))
+ * Round r = 0, 1, ... has three phases:
+ *   1. diagonal:  for k in K_r ascending, step k over i, j in K_r;
+ *   2. panels:    for k in K_r ascending, step k over i in K_r, j not in K_r (row panel) and over i not in K_r,
+ *                 j in K_r (column panel); the two panels are independent given phase 1;
+ *   3. remainder: for i, j not in K_r, D[i][j] <- R(...R(R(D[i][j], t_k0), t_k0+1)..., t_klast), t_k =
+ *                 Map(D[i][k], D[k][j]), the k running over K_r ascending, the panels as phase 2 left them, and the
+ *                 accumulator SEEDED WITH D[i][j], never with the reduce's identity (a float (Multiply, Max)
+ *                 reliability matrix keeps its "no path" zeros; the plain product would seed with FLT_MIN).
+ * Map and R are the functors of the product, one rounding each: float at flags 0 uses fminf / fmaxf (FMNMX) for Min /
+ * Max, under MM_FLAG_EXACT the literal (a < b) ? a : b, as mm_kernel_enqueue() does.  Consequences:
+ *   - with exact arithmetic the result is the true closure whatever b is: integers without wrap, Min / Max / And
+ *     maps, and float or double data whose path sums are exact;
+ *   - with rounding Add / Multiply maps, each element is a path weight rounded in the order stated above;
+ *   - integer Add wraps modulo 2^32 (uint8_t modulo 256) exactly as in the product, so INT_MAX as "no edge" is the
+ *     caller's to avoid (use a bound whose sums do not wrap);
+ *   - a negative (improving) cycle gives whatever the definition gives; the caller detects it on the diagonal.
+ * Validation as mm_kernel_enqueue_witness() with K = M = N, in the same order and with the same codes (N % the memory
+ * width != 0 -> MM_ERR_SHAPE; batch and extent limits of the batched call), plus: reduce_op other than MM_OP_MIN /
+ * MM_OP_MAX -> MM_ERR_INVALID; MM_FLAG_TRANSPOSED_A, MM_FLAG_BATCH_SHARED_A or _B -> MM_ERR_INVALID.
+ * MM_FLAG_TF32X3 is ignored.  The call uses no scratch, so it can be captured into a CUDA graph without a reserve;
+ * per-call profiling records it like a semiring call (the whole call is main time).  It launches 3 kernels per block
+ * of indices (1 when N <= b). */
+MM_API int mm_kernel_enqueue_closure(mm_context *ctx, int dtype, int map_op, int reduce_op, int flags,
+                                     void *d_device, unsigned size_n, unsigned batch, void *cuda_stream);
+/* b of mm_kernel_enqueue_closure() for `dtype`; 0 for an unknown dtype. */
+MM_API unsigned mm_closure_block(int dtype);
+
 /* Per-phase device timing of enqueued work, for roofline accounting.  With profiling on, every
  * mm_kernel_enqueue()/mm_kernel_execute() records CUDA events on the launching stream around
  * (i) the operand-preparation kernels and (ii) the main compute kernel.  mm_context_profile_read()

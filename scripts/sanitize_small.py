@@ -220,6 +220,34 @@ for case in ACCUMULATE:
     ok = accumulate_naive.same(dt, c, accumulate_naive.reduce_once(dt, rd, c0, p, fm), rd)
     print("%-42s %s" % (name, "ok" if ok else "MISMATCH"), flush=True)
     bad += 0 if ok else 1
+# closures (mm_kernel_enqueue_closure): a ragged last block on the ring and the tile remainder kernels, one partial
+# block, and a batch; D must equal the test suite's restatement (tests/closure_naive.py).  These cases have run on an
+# H100 without compute-sanitizer so far.
+import closure_data  # noqa: E402
+import closure_naive  # noqa: E402
+
+CLOSURE = [
+    ("closure ring f32 addmin", G.FLOAT, G.ADD, G.MIN, 0, 2 * 128 + 16, 1),
+    ("closure ring i32 addmax batch", G.INT32, G.ADD, G.MAX, 0, 128 + 16, 2),
+    ("closure tile f64 exact minmax", G.DOUBLE, G.MIN, G.MAX, G.FLAG_EXACT, 2 * 128 + 8, 1),
+    ("closure tile u8 andmax", G.UINT8, G.AND, G.MAX, 0, 128 + 64, 1),
+    ("closure pivot only bf16 addmin", G.BFLOAT16, G.ADD, G.MIN, 0, 96, 1),
+]
+for name, dt, mp, rd, flags, n, batch in CLOSURE:
+    if only and only not in name:
+        continue
+    d = closure_data.case(dt, mp, rd, n, 3, exact=bool(flags & G.FLAG_EXACT), batch=batch)
+    with G.Context(0) as ctx:
+        dd = ctx.alloc(d.nbytes)
+        ctx.copy_to_device(dd, d)
+        ctx.enqueue_closure(dt, mp, rd, dd, n, batch, flags=flags)
+        c = np.empty_like(d)
+        ctx.copy_to_host(c, dd)
+        ctx.free(dd)
+    fm = dt == G.FLOAT and not flags & G.FLAG_EXACT
+    ok = closure_naive.sd.same(c, closure_naive.closure(dt, mp, rd, d, fmnmx=fm))
+    print("%-42s %s" % (name, "ok" if ok else "MISMATCH"), flush=True)
+    bad += 0 if ok else 1
 # the row-block split on one device listed twice: sliced upload of B, the gather kernel, host barriers
 if not only or "multi" in only:
     for dt, shape in ((G.FLOAT, (300, 128, 272)), (G.HALF, (257, 128, 288)), (G.DOUBLE, (130, 128, 136)),
