@@ -9,5 +9,5 @@
 
 namespace mm {
 using InstT = MM_INST_T;
-MM_INSTANTIATE_SEMIRING_CLOSURE(InstT, MM_INST_MAP)
+MM_INSTANTIATE_SEMIRING(SemiringClosure, InstT, MM_INST_MAP, MM_OP_MIN, MM_OP_MAX)
 }  // namespace mm

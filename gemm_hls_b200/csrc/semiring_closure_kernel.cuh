@@ -17,13 +17,13 @@
 // of k, so a step needs one barrier: a buffer is rewritten two steps later, after every thread has passed the barrier
 // that follows its last read.
 //
-// Phase 3 is the product kernels' main loop (semiring_ring_kernel / semiring_tile_kernel, same per-element order of
-// operations) with three differences: the accumulators start from the C tile instead of the reduce's identity, the
-// operands are the panels of D read in place with row pitch N (TMA views of the whole batch, or pointers), and the
-// k loop covers exactly K_r's width: a multiple of the memory width, so a partial last panel never feeds the
-// zero-filled part of a TMA box into a term.  The CTA tile is 128 x 128 = b x b, so the tiles of block row and block
-// column r are whole CTAs; they return at once (they would race with the panels they read).  The other tiles read
-// only the panels and their own elements, and write only their own.
+// Phase 3 runs the product kernels' main loops (semiring_ring_body / semiring_tile_body, so the per-element order of
+// operations is theirs) with a closure variant: the accumulators start from the C tile instead of the reduce's
+// identity, the operands are the panels of D read in place with row pitch N (TMA views of the whole batch, or
+// pointers), and the k loop covers exactly K_r's width: a multiple of the memory width, so a partial last panel never
+// feeds the zero-filled part of a TMA box into a term.  The CTA tile is 128 x 128 = b x b, so the tiles of block row
+// and block column r are whole CTAs; they return at once (they would race with the panels they read).  The other tiles
+// read only the panels and their own elements, and write only their own.
 #pragma once
 
 #include "semiring_kernel.cuh"
@@ -178,361 +178,136 @@ __global__ void __launch_bounds__(256, 1) semiring_closure_panel_kernel(T *__res
   }
 }
 
-// Phase 3, 4-byte types: the ring kernel's TMA ring over the column panel (A: rows of the tile, columns K_r) and the
-// row panel (B: rows K_r, columns of the tile), both views of the whole batch (batch * N rows of N elements).
+// Phase 3's variants: problem 0's C is D, with N x N problems; the term is ClosureTerm's; the loop covers at most b k;
+// the accumulators start from this thread's elements of the C tile, the reduce's identity outside it.
+//
+// The ring variant recomputes the addresses of its epilogue from an opaque copy of n, so that they are not kept alive
+// (or spilled) across the main loop: element (i, h) of the thread sits at at(C, ..., i, h, n).
+template <typename T, class Map, class Reduce>
+struct ClosureRingVariant : SemiringVariant<T, Map, Reduce, false, ClosureTerm<T, Map>> {
+  static constexpr bool kFinish = true;
+  static constexpr unsigned kMaxK = kClosureBlock;
+  template <typename P>
+  static __device__ __forceinline__ P *at(P *C, unsigned row0, unsigned col0, int tx, int ty, int i, int h,
+                                          unsigned nn) {
+    return C + size_t(row0 + ty * 4) * nn + col0 + tx * 4 + (unsigned((i / 4) * 64 + (i % 4)) * nn + h * 64);
+  }
+  static __device__ __forceinline__ bool in(unsigned row0, unsigned col0, int tx, int ty, int i, int h, unsigned nn) {
+    return row0 + ty * 4 + (i / 4) * 64 + (i % 4) < nn && col0 + tx * 4 + h * 64 < nn;
+  }
+
+  __device__ __forceinline__ void seed(T (&acc)[8][8], NoState (&)[8][8], const T *C, unsigned row0, unsigned col0,
+                                       int tx, int ty) {
+    const unsigned n = this->size_n;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        Quad<T> old;
+        if (in(row0, col0, tx, ty, i, h, n)) {
+          old = *reinterpret_cast<const Quad<T> *>(at(C, row0, col0, tx, ty, i, h, n));
+        } else {
+#pragma unroll
+          for (int q = 0; q < 4; ++q) old.v[q] = Reduce::identity();
+        }
+#pragma unroll
+        for (int q = 0; q < 4; ++q) acc[i][h * 4 + q] = old.v[q];
+      }
+    }
+  }
+
+  __device__ __forceinline__ void finish(const T (&acc)[8][8], NoState (&)[8][8], unsigned row0, unsigned col0,
+                                         int tx, int ty) {
+    unsigned n_epi;
+    asm volatile("mov.u32 %0, %1;" : "=r"(n_epi) : "r"(this->size_n));
+    T *C = this->C + size_t(blockIdx.z) * n_epi * n_epi;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        if (in(row0, col0, tx, ty, i, h, n_epi)) {
+          Quad<T> out;
+#pragma unroll
+          for (int q = 0; q < 4; ++q) out.v[q] = acc[i][h * 4 + q];
+          *reinterpret_cast<Quad<T> *>(at(C, row0, col0, tx, ty, i, h, n_epi)) = out;
+        }
+      }
+    }
+  }
+};
+
+// The tile variant takes the body's C-tile seed and store; uint8_t with an And Map keeps the k loop rolled and loads
+// the next tile of the column panel late (ClosureRolledK).
+template <typename T, class Map, class Reduce>
+struct ClosureTileVariant : SemiringVariant<T, Map, Reduce, false, ClosureTerm<T, Map>> {
+  static constexpr bool kRolledK = ClosureRolledK<T, Map>::value, kLateA = kRolledK, kSeedC = true;
+  static constexpr unsigned kMaxK = kClosureBlock;
+};
+
+// Phase 3, 4-byte types: the ring's main loop over the column panel (A: rows of the tile, columns K_r) and the row
+// panel (B: rows K_r, columns of the tile), both read through views of the whole batch (batch * N rows of N elements).
 template <typename T, class Map, class Reduce>
 __global__ void __launch_bounds__(256, 2)
 semiring_closure_ring_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                              T *__restrict__ D, unsigned n, unsigned r) {
-  static_assert(sizeof(T) == 4, "ring variant: 4-byte element types");
-  using Cfg = SemiringRing;
-  using Term = ClosureTerm<T, Map>;
-  constexpr int BM = Cfg::BM, BN = Cfg::BN, BK = Cfg::BK, STAGES = Cfg::STAGES;
   if (blockIdx.x == r || blockIdx.y == r) return;  // block row / column r: the panels themselves
-  T *C = D + size_t(blockIdx.z) * n * n;
-  const unsigned k0 = r * kClosureBlock, p_row0 = blockIdx.z * n;
-
-  extern __shared__ unsigned char smem_raw[];
-  const uint32_t smem0 = (ptx::smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t full0 = smem0 + STAGES * Cfg::STAGE_BYTES, empty0 = full0 + 8 * STAGES;
-
-  const int tid = threadIdx.x, lane = tid % 32;
-  const int tx = tid % 16;  // column quad index
-  const int ty = tid / 16;  // row quad index
-  const unsigned row0 = blockIdx.y * BM, col0 = blockIdx.x * BN;
-  const unsigned k_tiles = min(kClosureBlock, n - k0) / BK;  // K_r's width is a multiple of BK: no zero-filled k
-
-  if (tid == 0) {
-    ptx::prefetch_tensormap(&tmap_a);
-    ptx::prefetch_tensormap(&tmap_b);
-    for (int s = 0; s < STAGES; ++s) {
-      ptx::mbar_init(full0 + 8 * s, 1);
-      ptx::mbar_init(empty0 + 8 * s, Cfg::THREADS / 32);
-    }
-    ptx::fence_mbar_init();
-  }
-  __syncthreads();
-
-  auto load_tile = [&](unsigned kt) {
-    const int stage = kt % STAGES;
-    if (kt >= STAGES) ptx::mbar_wait(empty0 + 8 * stage, ((kt / STAGES) - 1) & 1);
-    const uint32_t as = smem0 + stage * Cfg::STAGE_BYTES, bs = as + Cfg::A_BYTES, bar = full0 + 8 * stage;
-    ptx::mbar_arrive_expect_tx(bar, Cfg::STAGE_BYTES);
-    ptx::tma_load_2d(as, &tmap_a, bar, int32_t(k0 + kt * BK), int32_t(p_row0 + row0), ptx::L2_EVICT_NORMAL);
-    ptx::tma_load_2d(bs, &tmap_b, bar, int32_t(col0), int32_t(p_row0 + k0 + kt * BK), ptx::L2_EVICT_NORMAL);
-  };
-  if (tid == 0) {
-    for (unsigned kt = 0; kt < unsigned(Cfg::AHEAD) && kt < k_tiles; ++kt) load_tile(kt);
-  }
-
-  // The seed: this thread's elements of the C tile, in the store's layout (rows past N are never stored).  Element
-  // (i, h) of the thread sits at c_thr(n) + c_off(i, h, n).  The epilogue recomputes the addresses and masks from an
-  // opaque copy of n, so that they are not kept alive (or spilled) across the main loop.
-  auto c_thr = [&](unsigned nn) { return C + size_t(row0 + ty * 4) * nn + col0 + tx * 4; };
-  auto c_off = [&](int i, int h, unsigned nn) { return unsigned((i / 4) * 64 + (i % 4)) * nn + h * 64; };
-  auto c_in = [&](int i, int h, unsigned nn) {
-    return row0 + ty * 4 + (i / 4) * 64 + (i % 4) < nn && col0 + tx * 4 + h * 64 < nn;
-  };
-  T acc[8][8];
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      Quad<T> old;
-      if (c_in(i, h, n)) {
-        old = *reinterpret_cast<const Quad<T> *>(c_thr(n) + c_off(i, h, n));
-      } else {
-#pragma unroll
-        for (int q = 0; q < 4; ++q) old.v[q] = Reduce::identity();
-      }
-#pragma unroll
-      for (int q = 0; q < 4; ++q) acc[i][h * 4 + q] = old.v[q];
-    }
-  }
-
-  const int r_lo = ty * 4, r_hi = 64 + ty * 4;
-
-  for (unsigned kt = 0; kt < k_tiles; ++kt) {
-    const int stage = kt % STAGES;
-    if (tid == 0 && kt + Cfg::AHEAD < k_tiles) load_tile(kt + Cfg::AHEAD);
-    ptx::mbar_wait(full0 + 8 * stage, (kt / STAGES) & 1);
-    const unsigned char *as = smem_raw + (smem0 - ptx::smem_u32(smem_raw)) + stage * Cfg::STAGE_BYTES;
-    const T *bs = reinterpret_cast<const T *>(as + Cfg::A_BYTES);
-
-#pragma unroll
-    for (int c = 0; c < BK / 4; ++c) {
-      T a4[8][4];
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const int rr = (i < 4 ? r_lo : r_hi) + (i % 4);
-        const Quad<T> q = *reinterpret_cast<const Quad<T> *>(as + rr * 64 + c * 16);
-#pragma unroll
-        for (int v = 0; v < 4; ++v) a4[i][v] = Term::prep(q.v[v]);
-      }
-#pragma unroll
-      for (int kp = 0; kp < 4; kp += 2) {
-        const int kk = c * 4 + kp;
-        T bf[2][8];
-#pragma unroll
-        for (int u = 0; u < 2; ++u) {
-          const Quad<T> b0 = *reinterpret_cast<const Quad<T> *>(bs + (kk + u) * BN + tx * 4);
-          const Quad<T> b1 = *reinterpret_cast<const Quad<T> *>(bs + (kk + u) * BN + 64 + tx * 4);
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            bf[u][q] = Term::prep(b0.v[q]);
-            bf[u][4 + q] = Term::prep(b1.v[q]);
-          }
-        }
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            acc[i][j] = Reduce::Apply(Reduce::Apply(acc[i][j], Term::apply(a4[i][kp], bf[0][j])),
-                                      Term::apply(a4[i][kp + 1], bf[1][j]));
-          }
-        }
-      }
-    }
-    __syncwarp();
-    if (lane == 0) ptx::mbar_arrive(empty0 + 8 * stage);
-  }
-
-  unsigned n_epi;
-  asm volatile("mov.u32 %0, %1;" : "=r"(n_epi) : "r"(n));
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      if (c_in(i, h, n_epi)) {
-        Quad<T> out;
-#pragma unroll
-        for (int q = 0; q < 4; ++q) out.v[q] = acc[i][h * 4 + q];
-        *reinterpret_cast<Quad<T> *>(c_thr(n_epi) + c_off(i, h, n_epi)) = out;
-      }
-    }
-  }
+  const unsigned k0 = r * kClosureBlock;  // K_r's width, min(b, n - k0), is a multiple of BK: no zero-filled k
+  semiring_ring_body(ClosureRingVariant<T, Map, Reduce>{{D, n, n}}, tmap_a, 1u, k0, tmap_b, 1u, n, k0);
 }
 
-// Phase 3, the other types: the tile kernel's scheme.  The column panel is read through registers (rows clamped to
-// N - 1, never stored), transposed into shared memory; the row panel arrives by TMA from the view of the whole batch.
+// Phase 3, the other types: the tile's main loop.  The column panel (row i of problem 0 at D + k0 + i * n) is read
+// through registers, rows clamped to N - 1 (never stored); the row panel arrives by TMA from the view of the batch.
 template <typename T, class Map, class Reduce>
 __global__ void __launch_bounds__(256, 1)
 semiring_closure_tile_kernel(const __grid_constant__ CUtensorMap tmap_b, T *__restrict__ D, unsigned n, unsigned r) {
-  using Cfg = SemiringTile<T>;
-  using Term = ClosureTerm<T, Map>;
-  constexpr int BM = Cfg::BM, BN = Cfg::BN, BK = Cfg::BK, VEC = Cfg::VEC;
-  constexpr int LDA = Cfg::LDA, LDB = Cfg::LDB;
   if (blockIdx.x == r || blockIdx.y == r) return;
-  T *C = D + size_t(blockIdx.z) * n * n;
-  const unsigned k0 = r * kClosureBlock, b_k0 = blockIdx.z * n + k0;
-  const T *A = C + k0;  // the column panel: row i at A + i * n
-
-  extern __shared__ __align__(128) unsigned char smem_raw[];
-  T *As = reinterpret_cast<T *>(smem_raw);
-  T *Bs = reinterpret_cast<T *>(smem_raw + Cfg::A_BYTES);
-  const uint32_t bar0 = ptx::smem_u32(smem_raw + Cfg::A_BYTES + 2 * Cfg::B_TILE_BYTES);
-
-  const int tid = threadIdx.x;
-  const int tx = tid % 16;
-  const int ty = tid / 16;
-  const size_t row0 = size_t(blockIdx.y) * BM;
-  const size_t col0 = size_t(blockIdx.x) * BN;
-
-  T acc[8][8];
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    const size_t row = row0 + (i / 4) * 64 + ty * 4 + (i % 4);
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const size_t col = col0 + h * 64 + tx * 4;
-      Quad<T> old;
-      if (row < n && col + 4 <= n) {
-        old = *reinterpret_cast<const Quad<T> *>(C + row * n + col);
-      } else {
-#pragma unroll
-        for (int q = 0; q < 4; ++q) old.v[q] = Reduce::identity();
-      }
-#pragma unroll
-      for (int q = 0; q < 4; ++q) acc[i][h * 4 + q] = old.v[q];
-    }
-  }
-
-  Chunk16<T> a_stage[Cfg::CHUNKS_PER_THREAD];
-
-  if (tid == 0) {
-    ptx::prefetch_tensormap(&tmap_b);
-    ptx::mbar_init(bar0, 1);
-    ptx::mbar_init(bar0 + 8, 1);
-    ptx::fence_mbar_init();
-  }
-  __syncthreads();
-  auto load_b_tma = [&](int buf, unsigned kk0) {
-    if (tid == 0) {
-      ptx::mbar_arrive_expect_tx(bar0 + 8 * buf, uint32_t(Cfg::B_TILE_BYTES));
-      ptx::tma_load_2d(ptx::smem_u32(Bs + buf * BK * LDB), &tmap_b, bar0 + 8 * buf, int32_t(col0), int32_t(b_k0 + kk0),
-                       ptx::L2_EVICT_NORMAL);
-    }
-  };
-  auto load_global = [&](unsigned kk0) {
-#pragma unroll
-    for (int i = 0; i < Cfg::CHUNKS_PER_THREAD; ++i) {
-      const int c = tid + i * Cfg::THREADS;
-      const int rr = c / Cfg::A_CHUNKS_PER_ROW;
-      const int part = c % Cfg::A_CHUNKS_PER_ROW;
-      size_t row = row0 + rr;
-      if (row >= n) row = n - 1;
-      a_stage[i] = *reinterpret_cast<const Chunk16<T> *>(A + row * n + kk0 + part * VEC);
-    }
-  };
-  auto store_shared = [&](int buf) {
-    T *as = As + buf * BK * LDA;
-#pragma unroll
-    for (int i = 0; i < Cfg::CHUNKS_PER_THREAD; ++i) {
-      const int c = tid + i * Cfg::THREADS;
-      const int rr = c / Cfg::A_CHUNKS_PER_ROW;
-      const int part = c % Cfg::A_CHUNKS_PER_ROW;
-#pragma unroll
-      for (int v = 0; v < VEC; ++v) as[(part * VEC + v) * LDA + rr] = a_stage[i].v[v];
-    }
-  };
-
-  const unsigned k_tiles = min(kClosureBlock, n - k0) / BK;  // a multiple of the memory width BK
-  load_b_tma(0, 0);
-  load_global(0);
-  store_shared(0);
-  __syncthreads();
-  ptx::mbar_wait(bar0, 0);
-
-  for (unsigned kt = 0; kt < k_tiles; ++kt) {
-    const int buf = kt & 1;
-    constexpr bool kRolled = ClosureRolledK<T, Map>::value;
-    if (kt + 1 < k_tiles) {
-      load_b_tma(buf ^ 1, (kt + 1) * BK);
-      if (!kRolled) load_global((kt + 1) * BK);
-    }
-    const T *as = As + buf * BK * LDA;
-    const T *bs = Bs + buf * BK * LDB;
-    constexpr int KK_UNROLL = ClosureRolledK<T, Map>::value ? 1 : BK / 2;
-#pragma unroll KK_UNROLL
-    for (int kk = 0; kk < BK; kk += 2) {
-      T af[2][8], bf[2][8];
-#pragma unroll
-      for (int u = 0; u < 2; ++u) {
-        const Quad<T> a0 = *reinterpret_cast<const Quad<T> *>(as + (kk + u) * LDA + ty * 4);
-        const Quad<T> a1 = *reinterpret_cast<const Quad<T> *>(as + (kk + u) * LDA + 64 + ty * 4);
-        const Quad<T> b0 = *reinterpret_cast<const Quad<T> *>(bs + (kk + u) * LDB + tx * 4);
-        const Quad<T> b1 = *reinterpret_cast<const Quad<T> *>(bs + (kk + u) * LDB + 64 + tx * 4);
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          af[u][q] = Term::prep(a0.v[q]);
-          af[u][4 + q] = Term::prep(a1.v[q]);
-          bf[u][q] = Term::prep(b0.v[q]);
-          bf[u][4 + q] = Term::prep(b1.v[q]);
-        }
-      }
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          acc[i][j] = Reduce::Apply(Reduce::Apply(acc[i][j], Term::apply(af[0][i], bf[0][j])),
-                                    Term::apply(af[1][i], bf[1][j]));
-        }
-      }
-    }
-    if (kt + 1 < k_tiles) {
-      if (kRolled) load_global((kt + 1) * BK);
-      store_shared(buf ^ 1);
-    }
-    __syncthreads();
-    if (kt + 1 < k_tiles) ptx::mbar_wait(bar0 + 8 * (buf ^ 1), ((kt + 1) >> 1) & 1u);
-  }
-
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    const size_t row = row0 + (i / 4) * 64 + ty * 4 + (i % 4);
-    if (row >= n) continue;
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const size_t col = col0 + h * 64 + tx * 4;
-      if (col + 4 <= n) {
-        Quad<T> out;
-#pragma unroll
-        for (int q = 0; q < 4; ++q) out.v[q] = acc[i][h * 4 + q];
-        *reinterpret_cast<Quad<T> *>(C + row * n + col) = out;
-      }
-    }
-  }
+  const unsigned k0 = r * kClosureBlock;
+  semiring_tile_body(ClosureTileVariant<T, Map, Reduce>{{D, n, n}}, D + k0, 1u, n, false, tmap_b, 1u, n, k0);
 }
 
-// Host side: every round of the closure of `batch` packed N x N problems at d, on one stream.  Returns a cudaError_t
-// value as int.
+// Host side: every round of the closure of g.batch.count packed N x N problems at g.c, on one stream.  Phase 3 of a
+// 4-byte type always takes the ring (D is row-major and 16-byte aligned; there is no tile kernel for it).
 template <typename T, class Map, class Reduce>
-int launch_semiring_closure_typed(void *d, unsigned n, unsigned batch, cudaStream_t stream) {
-  T *D = static_cast<T *>(d);
-  const unsigned blocks = (n + kClosureBlock - 1) / kClosureBlock;
-  const size_t panel_smem = ClosureStep::diag_bytes<T>();
-  cudaError_t e = cudaFuncSetAttribute(semiring_closure_panel_kernel<T, Map, Reduce>,
-                                       cudaFuncAttributeMaxDynamicSharedMemorySize, int(panel_smem));
-  if (e != cudaSuccess) return static_cast<int>(e);
-  // both panels are read in place through a view of the whole batch: batch * N rows of N elements
-  const uint64_t rows = uint64_t(batch) * n;
-  CUtensorMap tmap_a, tmap_b;
-  size_t phase3_smem;
-  if constexpr (sizeof(T) == 4) {
-    using Cfg = SemiringRing;
-    phase3_smem = Cfg::SMEM_BYTES;
-    e = cudaFuncSetAttribute(semiring_closure_ring_kernel<T, Map, Reduce>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                             int(phase3_smem));
+struct SemiringClosure {
+  static int launch(const GemmArgs &g, unsigned *) {
+    T *D = static_cast<T *>(g.c);
+    const unsigned n = g.n, batch = g.batch.count, blocks = (n + kClosureBlock - 1) / kClosureBlock;
+    const size_t panel_smem = ClosureStep::diag_bytes<T>();
+    cudaError_t e = cudaFuncSetAttribute(semiring_closure_panel_kernel<T, Map, Reduce>,
+                                         cudaFuncAttributeMaxDynamicSharedMemorySize, int(panel_smem));
     if (e != cudaSuccess) return static_cast<int>(e);
-    if (encode_plain_2d(&tmap_a, d, sizeof(T), rows, n, Cfg::BM, Cfg::BK) != 0 ||
-        encode_plain_2d(&tmap_b, d, sizeof(T), rows, n, Cfg::BK, Cfg::BN) != 0) {
-      return static_cast<int>(cudaErrorInvalidValue);
-    }
-  } else {
-    using Cfg = SemiringTile<T>;
-    phase3_smem = Cfg::SMEM_BYTES;
-    if (encode_plain_2d(&tmap_b, d, sizeof(T), rows, n, Cfg::BK, Cfg::BN) != 0) {
-      return static_cast<int>(cudaErrorInvalidValue);
-    }
-  }
-  const dim3 block(ClosureStep::THREADS);
-  for (unsigned r = 0; r < blocks; ++r) {
-    semiring_closure_pivot_kernel<T, Map, Reduce><<<dim3(1, 1, batch), block, 0, stream>>>(D, n, r);
-    if (blocks == 1) break;  // no panels, no remainder
-    semiring_closure_panel_kernel<T, Map, Reduce><<<dim3(blocks, 2, batch), block, panel_smem, stream>>>(D, n, r);
-    const dim3 grid(blocks, blocks, batch);
+    const dim3 block(ClosureStep::THREADS);
+    auto rounds = [&](auto phase3) {
+      for (unsigned r = 0; r < blocks; ++r) {
+        semiring_closure_pivot_kernel<T, Map, Reduce><<<dim3(1, 1, batch), block, 0, g.stream>>>(D, n, r);
+        if (blocks == 1) break;  // no panels, no remainder
+        semiring_closure_panel_kernel<T, Map, Reduce><<<dim3(blocks, 2, batch), block, panel_smem, g.stream>>>(D, n, r);
+        phase3(r);
+      }
+    };
+    // both panels are read in place through a view of the whole batch: batch * N rows of N elements
+    const uint64_t rows = uint64_t(batch) * n;
     if constexpr (sizeof(T) == 4) {
-      semiring_closure_ring_kernel<T, Map, Reduce><<<grid, block, phase3_smem, stream>>>(tmap_a, tmap_b, D, n, r);
+      using Cfg = SemiringRing;
+      constexpr auto kernel = semiring_closure_ring_kernel<T, Map, Reduce>;
+      return launch_main_loop<T, Cfg::BN>(kernel, Cfg::SMEM_BYTES, true, D, rows, n, D, rows, n, n, n, batch,
+                                          [&](dim3 grid, const CUtensorMap &tmap_a, const CUtensorMap &tmap_b) {
+                                            rounds([&](unsigned r) {
+                                              kernel<<<grid, block, Cfg::SMEM_BYTES, g.stream>>>(tmap_a, tmap_b, D, n,
+                                                                                                  r);
+                                            });
+                                          });
     } else {
-      semiring_closure_tile_kernel<T, Map, Reduce><<<grid, block, phase3_smem, stream>>>(tmap_b, D, n, r);
+      using Cfg = SemiringTile<T>;
+      constexpr auto kernel = semiring_closure_tile_kernel<T, Map, Reduce>;
+      return launch_main_loop<T, Cfg::BN>(kernel, Cfg::SMEM_BYTES, false, D, rows, n, D, rows, n, n, n, batch,
+                                          [&](dim3 grid, const CUtensorMap &, const CUtensorMap &tmap_b) {
+                                            rounds([&](unsigned r) {
+                                              kernel<<<grid, block, Cfg::SMEM_BYTES, g.stream>>>(tmap_b, D, n, r);
+                                            });
+                                          });
     }
   }
-  return static_cast<int>(cudaGetLastError());
-}
-
-// One translation unit per (data type, map operator) instantiates the Min / Max reduces, plus the FMNMX pair for
-// float (semiring_closure_inst.cu compiled with -DMM_INST_T=<type> -DMM_INST_MAP=<MM_OP_*>).
-template <typename T, int MAP_OP>
-int launch_semiring_closure_for(int reduce_op, void *d, unsigned n, unsigned batch, cudaStream_t stream);
-
-#define MM_CLOSURE_CASE(REDOP)                                                                      \
-  if (reduce_op == REDOP)                                                                           \
-    return launch_semiring_closure_typed<T, typename OpSelect<T, MAP_OP>::type,                     \
-                                         typename OpSelect<T, REDOP>::type>(d, n, batch, stream);
-
-#define MM_INSTANTIATE_SEMIRING_CLOSURE(TYPE, MAPOP)                                                \
-  template <>                                                                                       \
-  int launch_semiring_closure_for<TYPE, MAPOP>(int reduce_op, void *d, unsigned n, unsigned batch,  \
-                                               cudaStream_t stream) {                               \
-    using T = TYPE;                                                                                 \
-    constexpr int MAP_OP = MAPOP;                                                                   \
-    MM_CLOSURE_CASE(MM_OP_MIN)                                                                      \
-    MM_CLOSURE_CASE(MM_OP_MAX)                                                                      \
-    if constexpr (std::is_same<T, float>::value) {                                                  \
-      MM_CLOSURE_CASE(MM_OP_MIN_FAST)                                                               \
-      MM_CLOSURE_CASE(MM_OP_MAX_FAST)                                                               \
-    }                                                                                               \
-    return -1;                                                                                      \
-  }
+};
 
 }  // namespace mm

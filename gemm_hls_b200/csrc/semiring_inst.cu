@@ -9,5 +9,6 @@
 
 namespace mm {
 using InstT = MM_INST_T;
-MM_INSTANTIATE_SEMIRING(InstT, MM_INST_MAP)
+MM_INSTANTIATE_SEMIRING(SemiringProduct, InstT, MM_INST_MAP,
+                        MM_OP_MULTIPLY, MM_OP_ADD, MM_OP_MIN, MM_OP_MAX, MM_OP_AND)
 }  // namespace mm

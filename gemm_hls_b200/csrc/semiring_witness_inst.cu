@@ -9,5 +9,5 @@
 
 namespace mm {
 using InstT = MM_INST_T;
-MM_INSTANTIATE_SEMIRING_WITNESS(InstT, MM_INST_MAP)
+MM_INSTANTIATE_SEMIRING(SemiringWitness, InstT, MM_INST_MAP, MM_OP_MIN, MM_OP_MAX)
 }  // namespace mm
