@@ -53,7 +53,8 @@ EXPORTS = ["mm_last_error", "mm_version", "mm_dtype_size", "mm_memory_width", "m
            "mm_kernel_enqueue_batched", "mm_context_reserve_batched", "mm_kernel_enqueue_witness",
            "mm_kernel_enqueue_accumulate", "mm_multi_create", "mm_multi_destroy", "mm_multi_device_count",
            "mm_multi_context", "mm_multi_peer_access", "mm_multi_partition", "mm_multi_gemm_host", "mm_multi_upload",
-           "mm_multi_execute", "mm_multi_download", "mm_kernel_enqueue_closure", "mm_closure_block"]
+           "mm_multi_execute", "mm_multi_download", "mm_kernel_enqueue_closure", "mm_closure_block",
+           "mm_kernel_enqueue_bool", "mm_kernel_enqueue_bool_closure"]
 
 
 class MMError(RuntimeError):
@@ -102,6 +103,8 @@ def lib():
         L.mm_kernel_enqueue_accumulate.argtypes = [vp, i, i, i, i, vp, vp, vp, u, u, u, u, vp]
         L.mm_kernel_enqueue_closure.argtypes = [vp, i, i, i, i, vp, u, u, vp]
         L.mm_closure_block.argtypes, L.mm_closure_block.restype = [i], u
+        L.mm_kernel_enqueue_bool.argtypes = [vp, i, vp, vp, vp, u, u, u, u, vp]
+        L.mm_kernel_enqueue_bool_closure.argtypes = [vp, i, vp, u, u, vp]
         L.mm_multi_create.argtypes = [i, ctypes.POINTER(i), ctypes.POINTER(vp)]
         L.mm_multi_destroy.argtypes = [vp]
         L.mm_multi_device_count.argtypes = [vp]
@@ -220,6 +223,19 @@ class Context:
         The diagonal is not initialised."""
         _check(lib().mm_kernel_enqueue_closure(self._h, dtype, map_op, reduce_op, flags, d_dev, n, batch,
                                                ctypes.c_void_p(stream) if stream else None))
+
+    def enqueue_bool(self, a_dev, b_dev, c_dev, n, k, m, batch=1, flags=0, stream=None):
+        """Bit-packed Boolean product C = A . B (C[i][j] = OR_k A[i][k] AND B[k][j]) for `batch` packed problems, on the
+        b1 tensor cores.  Each matrix is row-major with bit j % 8 of byte j / 8 for column j (numpy.packbits(...,
+        bitorder='little')); k and m must be multiples of 128."""
+        _check(lib().mm_kernel_enqueue_bool(self._h, flags, a_dev, b_dev, c_dev, n, k, m, batch,
+                                            ctypes.c_void_p(stream) if stream else None))
+
+    def enqueue_bool_closure(self, d_dev, n, batch=1, flags=0, stream=None):
+        """D <- its transitive closure (paths of one or more edges) in place, for `batch` packed bit-packed n x n
+        matrices (layout as enqueue_bool; n a multiple of 128).  The diagonal is not set reflexively."""
+        _check(lib().mm_kernel_enqueue_bool_closure(self._h, flags, d_dev, n, batch,
+                                                    ctypes.c_void_p(stream) if stream else None))
 
     def set_tuning(self, **knobs):
         """mm_context_set_tuning by name, e.g. ctx.set_tuning(cta_group=1, stages=4)."""

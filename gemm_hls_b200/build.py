@@ -22,7 +22,7 @@ FLAGS = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-Xcompiler", 
          "--expt-relaxed-constexpr"]
 
 SOURCES = ["capi.cu", "gemm_tcgen05.cu", "gemm_wgmma_bf16.cu", "gemm_wgmma_acc.cu", "gemm_dmma.cu", "gemm_dmma_acc.cu",
-           "semiring_dispatch.cu"]
+           "semiring_dispatch.cu", "gemm_wgmma_b1.cu", "bool_closure.cu"]
 # semiring_inst.cu, semiring_witness_inst.cu, semiring_accumulate_inst.cu and semiring_closure_inst.cu are compiled
 # once per (type, map operator): (object suffix, C type)
 INST_TYPES = [("f16", "__half"), ("f32", "float"), ("f64", "double"), ("i32", "int"),

@@ -213,6 +213,14 @@ int check_batch(unsigned batch, unsigned n, unsigned k, unsigned m) {
   return MM_OK;
 }
 
+// Bit matrices: K and M (the closure's N) multiples of 128, so that every row is a whole number of 16-byte words.
+int check_bool_shape(const char *what, unsigned x) {
+  if (x % 128 != 0) {
+    return fail(MM_ERR_SHAPE, std::string(what) + " (" + std::to_string(x) + ") must be a multiple of 128 bits.");
+  }
+  return MM_OK;
+}
+
 // Whether the byte ranges [x, x + x_bytes) and [y, y + y_bytes) share a byte.
 bool overlaps(const void *x, size_t x_bytes, const void *y, size_t y_bytes) {
   const uintptr_t x0 = reinterpret_cast<uintptr_t>(x), y0 = reinterpret_cast<uintptr_t>(y);
@@ -1034,6 +1042,63 @@ int mm_kernel_enqueue_closure(mm_context *ctx, int dtype, int map_op, int reduce
   if ((rc = begin_call(ctx, s, /*profile=*/true, &capture, &pe)) != MM_OK) return rc;
   if (pe) MM_CUDA_TRY(cudaEventRecord(pe[1], s));  // like a semiring call: no preparation
   if ((rc = mm::launch_semiring_closure(dtype, map_op, reduce_op, flags, d, n, batch, s)) != MM_OK) return rc;
+  if (pe) MM_CUDA_TRY(cudaEventRecord(pe[2], s));
+  return MM_OK;
+}
+
+int mm_kernel_enqueue_bool(mm_context *ctx, int flags, const void *a, const void *b, void *c, unsigned n, unsigned k,
+                           unsigned m, unsigned batch, void *cuda_stream) {
+  if (!ctx) return fail(MM_ERR_INVALID, "null context");
+  if (!a || !b || !c) return fail(MM_ERR_INVALID, "null matrix pointer");
+  if (n == 0 || k == 0 || m == 0) return fail(MM_ERR_INVALID, "matrix dimensions must be positive");
+  int rc;
+  if ((rc = check_bool_shape("K", k)) != MM_OK || (rc = check_bool_shape("M", m)) != MM_OK) return rc;
+  if ((rc = check_batch(batch, n, k, m)) != MM_OK) return rc;
+  if ((rc = check_device_alignment(a, b, c)) != MM_OK) return rc;
+  if (flags != 0) return fail(MM_ERR_INVALID, "flags is reserved and must be 0");
+  const size_t a_bytes = size_t(batch) * n * (k / 8), b_bytes = size_t(batch) * k * (m / 8);
+  const size_t c_bytes = size_t(batch) * n * (m / 8);
+  if (overlaps(c, c_bytes, a, a_bytes) || overlaps(c, c_bytes, b, b_bytes)) {
+    return fail(MM_ERR_INVALID, "C must not overlap A or B");
+  }
+  std::lock_guard<std::mutex> lock(ctx->mutex);
+  MM_CUDA_TRY(cudaSetDevice(ctx->device));
+  cudaStream_t s = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ctx->stream;
+  cudaStreamCaptureStatus capture;
+  cudaEvent_t *pe;
+  if ((rc = begin_call(ctx, s, /*profile=*/true, &capture, &pe)) != MM_OK) return rc;
+  // the scratch: B's K-major copy (b_bytes), then the GEMM's wave-barrier counter at the tail
+  const size_t need = b_bytes + mm::kTcgen05TailBytes;
+  if (need > ctx->scratch.bytes && capture != cudaStreamCaptureStatusNone) {
+    return fail(MM_ERR_INVALID, "the scratch cannot grow during stream capture: make a first call outside the capture");
+  }
+  if ((rc = ensure(ctx, ctx->scratch, need, ctx->captured)) != MM_OK) return rc;
+  if ((rc = mm::bool_transpose_b(b, ctx->scratch.ptr, k, m, batch, s)) != MM_OK) return rc;
+  if (pe) MM_CUDA_TRY(cudaEventRecord(pe[1], s));
+  rc = mm::bool_gemm(a, ctx->scratch.ptr, c, n, k, m, batch, ctx->tuning,
+                     mm::tcgen05_tile_sync(ctx->scratch.ptr, ctx->scratch.bytes), s);
+  if (rc != MM_OK) return rc;
+  if (pe) MM_CUDA_TRY(cudaEventRecord(pe[2], s));
+  return MM_OK;
+}
+
+int mm_kernel_enqueue_bool_closure(mm_context *ctx, int flags, void *d, unsigned n, unsigned batch, void *cuda_stream) {
+  if (!ctx) return fail(MM_ERR_INVALID, "null context");
+  if (!d) return fail(MM_ERR_INVALID, "null matrix pointer");
+  if (n == 0) return fail(MM_ERR_INVALID, "matrix dimensions must be positive");
+  int rc;
+  if ((rc = check_bool_shape("N", n)) != MM_OK) return rc;
+  if ((rc = check_batch(batch, n, n, n)) != MM_OK) return rc;
+  if ((rc = check_device_alignment(d, d, d)) != MM_OK) return rc;
+  if (flags != 0) return fail(MM_ERR_INVALID, "flags is reserved and must be 0");
+  std::lock_guard<std::mutex> lock(ctx->mutex);
+  MM_CUDA_TRY(cudaSetDevice(ctx->device));
+  cudaStream_t s = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ctx->stream;
+  cudaStreamCaptureStatus capture;
+  cudaEvent_t *pe;
+  if ((rc = begin_call(ctx, s, /*profile=*/true, &capture, &pe)) != MM_OK) return rc;
+  if (pe) MM_CUDA_TRY(cudaEventRecord(pe[1], s));  // no preparation: the whole call is main time
+  if ((rc = mm::bool_closure(d, n, batch, s)) != MM_OK) return rc;
   if (pe) MM_CUDA_TRY(cudaEventRecord(pe[2], s));
   return MM_OK;
 }

@@ -169,6 +169,15 @@ constexpr size_t kTcgen05TailBytes = 256;  // [wave-barrier counter, 256 B]
 int gather_b_rows(const void *const *parts, unsigned part_rows, void *dst, size_t elem_bytes, unsigned k, unsigned m,
                   cudaStream_t stream);
 
+// Bit-packed Boolean matrices (mm_kernel_enqueue_bool / _closure); every offset in bytes, rows of (columns / 8) bytes.
+// `batch` packed K x M bit matrices at b -> their M x K transposes at bt.  gemm_wgmma_b1.cu
+int bool_transpose_b(const void *b, void *bt, unsigned k, unsigned m, unsigned batch, cudaStream_t stream);
+// C[N x M] = A[N x K] . B'^T on the b1 wgmma, B' the M x K copy of bool_transpose_b.  gemm_wgmma_b1.cu
+int bool_gemm(const void *a, const void *bt, void *c, unsigned n, unsigned k, unsigned m, unsigned batch,
+              const Tuning &t, unsigned int *tile_sync, cudaStream_t stream);
+// `batch` packed N x N bit matrices at d -> their transitive closures, in place.  bool_closure.cu
+int bool_closure(void *d, unsigned n, unsigned batch, cudaStream_t stream);
+
 // DMMA (mma.sync m8n8k4 f64) GEMM for (Multiply, Add) double.  gemm_dmma.cu
 int launch_dmma(const GemmArgs &args);
 // The same with C <- C_old + product.  gemm_dmma_acc.cu

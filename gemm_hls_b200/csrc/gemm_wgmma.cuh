@@ -1,7 +1,7 @@
 // The wgmma tensor-core GEMM kernel (C = A' * B'^T, both operands K-major) and its host-side launch
 // machinery: tensor maps, run-time parameters and the per-variant launcher.  Shared by the translation
-// units that instantiate it: gemm_tcgen05.cu (tf32, f16, u8), gemm_wgmma_bf16.cu (bf16) and gemm_wgmma_acc.cu (the
-// accumulate kernels of every type).  The kernel's
+// units that instantiate it: gemm_tcgen05.cu (tf32, f16, u8), gemm_wgmma_bf16.cu (bf16), gemm_wgmma_b1.cu (bit-packed
+// Boolean) and gemm_wgmma_acc.cu (the accumulate kernels of every type).  The kernel's
 // structure is described at the top of gemm_tcgen05.cu.
 #pragma once
 
@@ -179,6 +179,94 @@ struct GemmParams {
   const unsigned int *fits_a, *fits_b;
 };
 
+// The counts of a b1 wgmma fragment (ptx::wgmma) as bits, count > 0: w[i][chunk] = columns 32 chunk .. + 32 of the
+// lane's row i (of two), bit j % 32 for column j.  Each lane holds two columns of every eight of its rows; an OR over
+// the four lanes of a row (q = lane % 4) assembles every word in all four.
+template <int BN>
+__device__ __forceinline__ void pack_bit_words(const uint32_t (&acc)[BN / 2], uint32_t q, uint32_t (&w)[2][BN / 32]) {
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+#pragma unroll
+    for (int chunk = 0; chunk < BN / 32; ++chunk) {
+      uint32_t x = 0;
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+#pragma unroll
+        for (int c = 0; c < 2; ++c) x |= uint32_t(acc[4 * (4 * chunk + j) + 2 * i + c] != 0u) << (8 * j + 2 * q + c);
+      }
+      x |= __shfl_xor_sync(0xFFFFFFFFu, x, 1);
+      x |= __shfl_xor_sync(0xFFFFFFFFu, x, 2);
+      w[i][chunk] = x;
+    }
+  }
+}
+
+// The 32 x 32 bit block whose row l is `x` in lane l becomes its transpose: bit c of lane l's word = bit l of lane c's
+// word on entry.  Five exchange stages, each swapping the off-diagonal halves of every 2s x 2s sub-block.  Used by the
+// b1 preparation (gemm_wgmma_b1.cu) and the Boolean closure (bool_closure.cu) to make row-major bits K-major.
+__device__ __forceinline__ uint32_t warp_transpose32(uint32_t x, uint32_t lane) {
+  uint32_t m = 0x0000FFFFu;
+#pragma unroll
+  for (int s = 16; s > 0; s >>= 1, m ^= m << s) {
+    const uint32_t y = __shfl_xor_sync(0xFFFFFFFFu, x, s);
+    x = (lane & s) ? ((x & ~m) | ((y >> s) & m)) : ((x & ~(m << s)) | ((y & m) << s));
+  }
+  return x;
+}
+
+// b1 epilogue (mm_kernel_enqueue_bool): this warp's 16 rows x BN columns of C as bits, C[i][j] = count > 0.  C rows
+// are `cols` / 8 bytes; bit j % 8 of byte j / 8, least significant first.  A 128-column group of one row is 16
+// bytes, the narrowest TMA box and one 128-bit store, so the warp writes whole groups: through the staging buffer
+// and one TMA store of 16 rows x BN / 8 bytes (tma_store), or directly.
+template <typename G, int BN>
+__device__ __forceinline__ void store_bit_tile(const uint32_t (&acc)[BN / 2], const CUtensorMap &tmap_c,
+                                               unsigned char *__restrict__ C, const GemmParams &p, const TileCoord &tc,
+                                               uint32_t cta_rank, uint32_t cwarp, uint32_t lane, uint32_t buf) {
+  constexpr int GROUPS = BN / 128;  // 128-column groups per row of the tile
+  const uint32_t row0 = tc.r * G::TILE_ROWS + cta_rank * BLOCK_M + cwarp * EPI_ROWS;
+  const uint32_t r_in = lane / 4, q = lane % 4;
+  uint32_t w[2][BN / 32];
+  pack_bit_words<BN>(acc, q, w);
+  const uint32_t row_bytes = p.cols / 8;
+  if (p.tma_store) {
+    if (row0 >= p.rows) return;  // warp-uniform
+    constexpr uint32_t PITCH = BN / 8;
+    if (lane == 0) ptx::tma_store_wait_read<0>();  // the previous block has left the buffer
+    __syncwarp();
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+#pragma unroll
+      for (int g = 0; g < GROUPS; ++g) {
+        if (q == uint32_t(i * GROUPS + g)) {
+          ptx::st_shared_v4(buf + (r_in + 8 * i) * PITCH + 16 * g, w[i][4 * g], w[i][4 * g + 1], w[i][4 * g + 2],
+                            w[i][4 * g + 3]);
+        }
+      }
+    }
+    ptx::fence_proxy_async_smem();
+    __syncwarp();
+    if (lane == 0) {
+      // clipped to rows x cols of this problem by the map
+      ptx::tma_store_3d(&tmap_c, buf, int32_t(tc.c * (BN / 8)), int32_t(row0), int32_t(tc.prob));
+      ptx::tma_store_commit();
+    }
+  } else {
+    unsigned char *Cp = C + size_t(tc.prob) * p.rows * row_bytes;
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const uint32_t row = row0 + r_in + 8 * i;
+#pragma unroll
+      for (int g = 0; g < GROUPS; ++g) {
+        const uint32_t col = tc.c * BN + 128 * g;
+        if (q == uint32_t(i * GROUPS + g) && row < p.rows && col < p.cols) {
+          *reinterpret_cast<uint4 *>(Cp + size_t(row) * row_bytes + col / 8) =
+              make_uint4(w[i][4 * g], w[i][4 * g + 1], w[i][4 * g + 2], w[i][4 * g + 3]);
+        }
+      }
+    }
+  }
+}
+
 // C[rows x cols] = A'[rows x k] * B'^T ; A' (rows x k) and B' (cols x k) K-major.  CG == 2 must be
 // launched with cluster dimension (2, 1, 1).  ACC: C = C_old + A'B'^T, the add applied to the rounded product in
 // the epilogue (gemm_wgmma_accumulate_kernel); nothing else differs.
@@ -190,7 +278,8 @@ __device__ __forceinline__ void gemm_wgmma_body(const CUtensorMap &tmap_a, const
                                                 const CUtensorMap &tmap_a16, const CUtensorMap &tmap_b16,
                                                 const CUtensorMap &tmap_c, TOut *__restrict__ C, const GemmParams &p) {
   using G = Geo<CG, BN>;
-  constexpr int ELEM_BYTES = (KIND == ptx::KIND_TF32) ? 4 : (KIND == ptx::KIND_I8 ? 1 : 2);  // f16, bf16: 2
+  // f16, bf16: 2; b1 moves its bits as bytes, as u8 does
+  constexpr int ELEM_BYTES = (KIND == ptx::KIND_TF32) ? 4 : ((KIND == ptx::KIND_I8 || KIND == ptx::KIND_B1) ? 1 : 2);
   constexpr int BLOCK_K_ELEMS = BLOCK_K_BYTES / ELEM_BYTES;
   const int STAGES = int(p.num_stages);
   const uint32_t rows = p.rows, cols = p.cols;
@@ -331,6 +420,11 @@ __device__ __forceinline__ void gemm_wgmma_body(const CUtensorMap &tmap_a, const
         mainloop(std::integral_constant<int, ptx::KIND_F16>{}, num_kb16);
       } else {
         mainloop(std::integral_constant<int, KIND>{}, num_kb);
+      }
+
+      if constexpr (KIND == ptx::KIND_B1) {
+        store_bit_tile<G, BN>(acc, tmap_c, C, p, tc, cta_rank, cwarp, lane, buf);
+        continue;
       }
 
       // ---- epilogue: this warp's 16 rows x BN columns ----

@@ -283,6 +283,36 @@ MM_API int mm_kernel_enqueue_closure(mm_context *ctx, int dtype, int map_op, int
 /* b of mm_kernel_enqueue_closure() for `dtype`; 0 for an unknown dtype. */
 MM_API unsigned mm_closure_block(int dtype);
 
+/* ---- bit-packed Boolean matrices: products and transitive closure on the b1 tensor cores -----------------------
+ * Layout: an R x L Boolean matrix is stored bit-packed and row-major, element (i, j) = bit j % 8 (least significant
+ * first) of byte i*L/8 + j/8, i.e. numpy.packbits(X, axis=-1, bitorder='little').  A batch is packed: problem p starts
+ * at byte p*R*L/8.  Every offset is 64-bit.
+ *
+ * mm_kernel_enqueue_bool(): C[p][i][j] = 1 iff some k has A[p][i][k] = B[p][k][j] = 1, for A N x K, B K x M (row-major)
+ * and C N x M, on wgmma m64nNk256 .b1.and.popc: exact counts of A AND B, stored as count > 0.  Asynchronous like the
+ * other enqueue entries; every bit of C is written (with M a multiple of 128, rows of C have no padding bits).  It
+ * keeps a K-major copy of B (batch*K*M/8 bytes) in the context's scratch, sized by a first call outside a stream
+ * capture; per-call profiling records that copy as preparation and the product as main time.  The wgmma tuning knobs
+ * apply (cta_group, block_n, stages, raster_rows, tile_sync, tma_store, l2_policy) and give the same bits.
+ *
+ * mm_kernel_enqueue_bool_closure(): `batch` packed N x N matrices D become D+ in place: D+[i][j] = 1 iff a path of one
+ * or more edges leads from i to j.  The diagonal is 1 exactly where i lies on a cycle (self-loops included): the call
+ * does not set the reflexive diagonal, as mm_kernel_enqueue_closure() does not initialise it.  The result is
+ * BIT-IDENTICAL to mm_kernel_enqueue_closure(MM_DTYPE_UINT8, MM_OP_AND, MM_OP_MAX, 0, ...) on the unpacked 0/1 bytes,
+ * after packing.  Blocked Floyd–Warshall; the block size cannot be observed in the result.  No scratch: it can be
+ * captured into a CUDA graph without a prior call.  Per-call profiling records the whole call as main time.
+ *
+ * Validation, in this order: null context or pointer, or N, K or M equal to 0 -> MM_ERR_INVALID; K or M (closure: N)
+ * not a multiple of 128 -> MM_ERR_SHAPE; the batch limits of mm_kernel_enqueue_batched(); pointers not 16-byte aligned
+ * -> MM_ERR_INVALID; flags != 0 (reserved) -> MM_ERR_INVALID; product: C's bytes overlapping A's or B's ->
+ * MM_ERR_INVALID.  mm_kernel_launch_count(), mm_kernel_path() and the tuning enum do not describe these calls.
+ * Callers detect the feature by these symbols. */
+MM_API int mm_kernel_enqueue_bool(mm_context *ctx, int flags, const void *a_device, const void *b_device,
+                                  void *c_device, unsigned size_n, unsigned size_k, unsigned size_m,
+                                  unsigned batch, void *cuda_stream);
+MM_API int mm_kernel_enqueue_bool_closure(mm_context *ctx, int flags, void *d_device, unsigned size_n,
+                                          unsigned batch, void *cuda_stream);
+
 /* Per-phase device timing of enqueued work, for roofline accounting.  With profiling on, every
  * mm_kernel_enqueue()/mm_kernel_execute() records CUDA events on the launching stream around
  * (i) the operand-preparation kernels and (ii) the main compute kernel.  mm_context_profile_read()

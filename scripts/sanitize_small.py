@@ -248,6 +248,39 @@ for name, dt, mp, rd, flags, n, batch in CLOSURE:
     ok = closure_naive.sd.same(c, closure_naive.closure(dt, mp, rd, d, fmnmx=fm))
     print("%-42s %s" % (name, "ok" if ok else "MISMATCH"), flush=True)
     bad += 0 if ok else 1
+# bit-packed Boolean products and closures (mm_kernel_enqueue_bool / _closure) at ragged shapes: partial row tiles, a
+# partial last column tile, a batch, and a closure whose last block of indices is half full; against tests/bool_naive.py.
+import bool_naive  # noqa: E402
+
+BOOL = [("bool product 129x384x384", 129, 384, 384, 1), ("bool product 1x1152x640 batch", 1, 1152, 640, 2),
+        ("bool closure 384", 384, 384, 384, 1), ("bool closure 640 batch", 640, 640, 640, 2)]
+for name, n, k, m, batch in BOOL:
+    if only and only not in name:
+        continue
+    with G.Context(0) as ctx:
+        if "closure" in name:
+            d = np.stack([bool_naive.hamiltonian_cycle(n, p) | bool_naive.random_bits((n, n), 0.002, p)
+                          for p in range(batch)])
+            dd = ctx.alloc(d.size // 8)
+            ctx.copy_to_device(dd, bool_naive.pack(d))
+            ctx.enqueue_bool_closure(dd, n, batch)
+            want = np.stack([bool_naive.closure(x) for x in d])
+        else:
+            a = bool_naive.random_bits((batch, n, k), 0.01, 1)
+            b = bool_naive.random_bits((batch, k, m), 0.01, 2)
+            da, db, dd = ctx.alloc(a.size // 8), ctx.alloc(b.size // 8), ctx.alloc(batch * n * m // 8)
+            ctx.copy_to_device(da, bool_naive.pack(a))
+            ctx.copy_to_device(db, bool_naive.pack(b))
+            ctx.enqueue_bool(da, db, dd, n, k, m, batch)
+            want = bool_naive.product(a, b)
+            ctx.free(da)
+            ctx.free(db)
+        c = np.empty((batch, n, m // 8), np.uint8)
+        ctx.copy_to_host(c, dd)
+        ctx.free(dd)
+    ok = np.array_equal(bool_naive.unpack(c, m), want)
+    print("%-42s %s" % (name, "ok" if ok else "MISMATCH"), flush=True)
+    bad += 0 if ok else 1
 # the row-block split on one device listed twice: sliced upload of B, the gather kernel, host barriers
 if not only or "multi" in only:
     for dt, shape in ((G.FLOAT, (300, 128, 272)), (G.HALF, (257, 128, 288)), (G.DOUBLE, (130, 128, 136)),
